@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""bench.py -- stage-1 structural indexing throughput on B200 (BASELINE.json metric).
+"""bench.py -- stage-1 structural indexing throughput on H100 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config NAME] [--check]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config NAME] [--check] [--dump-outputs DIR]
 
 One "step" = one stage-1 pass (structural indexing + UTF-8 validation) over one batch of synthetic input per GPU.
 
 Configurations (`--config`, BASELINE.json `configs`):
-  stage1_64m   (default) configs[1]: synthetic 64 MiB random-structure JSON, stage 1 on 1xB200.  At N>1 every rank
+  stage1_64m   (default) configs[1]: synthetic 64 MiB random-structure JSON, stage 1 on 1xH100.  At N>1 every rank
                holds one 64 MiB shard of ONE N x 64 MiB document (a JSON array cut after line feeds, so no shard is a
                document of its own); every step is a sharded pass through sjb200_stage1_sharded: the scan kernel itself
                stores each shard's {count, state, transducer, flags} record into every rank's exchange window over
@@ -17,6 +17,8 @@ Configurations (`--config`, BASELINE.json `configs`):
   concat_8g    configs[4]: twitter + citm repeated to 8 GiB, 8 shards of ~1 GiB with 64-bit index bases, round-robin
                over the N ranks
   tokens_64m   SURVEY.md 8(f) row 4 (not a BASELINE config): stage-2-lite (sjb200_tokens_dev) on the 64 MiB document
+`--dump-outputs DIR` (default config) writes what the last timed step computed as DIR/<name>.npy (float64): the
+[error, n_structural_indexes] pair and 2 Mi index words (over all ranks) at seeded positions, with the positions: 32 MiB.
 `--check` runs the parity gate of the multi-rank path on adversarial cuts (mid-row, mid-string: carry-in != 0, second
 round, re-scans) through the real IPC / NCCL plumbing and prints one JSON line; exit code 1 on a mismatch.
 
@@ -48,8 +50,8 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 DOC_BYTES = 64 << 20
-ROTATE = 4  # distinct 64 MiB inputs used round-robin: 256 MiB > 126 MB of L2, so no step finds its input in L2
-METRIC = "stage1 GB/s (bytes in / s) vs HBM roofline at 1/2/4/8 B200; CPU ref GB/s"
+ROTATE = 4  # distinct 64 MiB inputs used round-robin: 256 MiB > 50 MB of L2, so no step finds its input in L2
+METRIC = "stage1 GB/s (bytes in / s) vs HBM roofline at 1/2/4/8 H100; CPU ref GB/s"
 UNIT = "GB/s"
 PLUGIN = os.path.join(ROOT, "simdjson_b200", "plugin", "libsimdjson_b200.so")
 KERNEL_SOURCES = ["sjb200_scan4.cuh", "sjb200_bits.cuh", "sjb200_simt.cuh", "sjb200_params.h", "sjb200_kernels.cu", "sjb200_utf8.cuh"]
@@ -57,8 +59,8 @@ KERNEL_SOURCES = ["sjb200_scan4.cuh", "sjb200_bits.cuh", "sjb200_simt.cuh", "sjb
 
 def workload_name(world):
     if world == 1:
-        return "synthetic 64 MiB random-structure JSON, stage1 index on 1xB200 (BASELINE.json configs[1])"
-    return f"synthetic {world} x 64 MiB random-structure JSON, stage1 sharded by byte range over {world}xB200 (BASELINE.json configs[1] per GPU)"
+        return "synthetic 64 MiB random-structure JSON, stage1 index on 1xH100 (BASELINE.json configs[1])"
+    return f"synthetic {world} x 64 MiB random-structure JSON, stage1 sharded by byte range over {world}xH100 (BASELINE.json configs[1] per GPU)"
 
 
 def peaks():
@@ -68,7 +70,7 @@ def peaks():
             return float(json.load(open(path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:  # noqa: BLE001
             pass
-    return 6650.0, "fallback (B200_PROFILING.md: 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s)"
 
 
 def kernel_source_hash():
@@ -291,16 +293,17 @@ def cpu_baseline(doc, steps=3):
         ref = O.Ref("")
         threads = max(1, min(cores, int(os.environ.get("SJB200_REF_THREADS", cores))))
         best1, mean1, _ = ref.time_rounds(0, doc, 0, 1, 1, 3)
-        bestn, meann, err = ref.time_rounds(0, doc, 0, threads, 1, max(2, steps))
+        bestn, meann, err = ref.time_rounds(0, doc, 0, threads, 1, steps)
         return {"value": round(threads * len(doc) / meann / 1e9, 3), "unit": UNIT, "cores": threads, "kind": "reference",
                 "value_best_round": round(threads * len(doc) / bestn / 1e9, 3), "one_core": round(len(doc) / mean1 / 1e9, 3),
-                "sample": f"{ref.name} kernel; {threads} pre-spawned threads x one private {len(doc) >> 20} MiB document each, mean of {max(2, steps)} rounds after 1 warm-up round",
+                "sample": f"{ref.name} kernel; {threads} pre-spawned threads x one private {len(doc) >> 20} MiB document each, mean of {steps} rounds after 1 warm-up round",
                 "error_code": err}
     port = O.Port()
     t0 = time.perf_counter()
-    port.stage1(doc[: 16 << 20], 0)
-    dt = time.perf_counter() - t0
-    return {"value": round((16 << 20) / dt / 1e9, 3), "unit": UNIT, "cores": 1, "kind": "port", "sample": "scalar C port, 16 MiB prefix, one pass"}
+    for _ in range(steps):
+        port.stage1(doc[: 16 << 20], 0)
+    dt = (time.perf_counter() - t0) / steps
+    return {"value": round((16 << 20) / dt / 1e9, 3), "unit": UNIT, "cores": 1, "kind": "port", "sample": f"scalar C port, 16 MiB prefix, mean of {steps} passes"}
 
 
 # =============================================================================== reference arm
@@ -310,7 +313,7 @@ def run_reference(args, rank, world):
     if rank != 0:
         return
     doc = make_doc(0)
-    cb = cpu_baseline(doc, steps=max(2, min(args.steps, 8)))
+    cb = cpu_baseline(doc, steps=args.steps)
     line = {
         "impl": "reference", "metric": METRIC, "value": cb["value"], "unit": UNIT, "n_gpus": args.gpus, "steps": args.steps, "warmup": args.warmup,
         "ms_per_step": round(len(doc) * cb["cores"] / (cb["value"] * 1e9) * 1e3, 3), "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u8",
@@ -340,6 +343,27 @@ def plugin_e2e(doc, iters, want_words=None):
     if want_words is not None:
         ok = bool(rc == 0 and np.array_equal(idx[: len(want_words)], want_words))
     return {"rc": rc, "n": int(n.value), "seconds_total": secs[0], "seconds_best": secs[1], "gpu_calls": int(calls.value), "parity": ok}
+
+
+# =============================================================================== --dump-outputs
+DUMP_WORDS = 2 << 20  # sampled index words over all ranks: two float64 arrays of this length in all, 32 MiB
+DUMP_RANGE = DOC_BYTES // 8  # positions are drawn from [0, DUMP_RANGE), whatever n is
+
+
+def dump_outputs(out_dir, d_idx, n, n_words, world, prefix=""):
+    """what the last timed step returned to its caller: (error, n) and its index words (n + 3 with the sentinels of a
+    single-GPU scan, n for a shard) at DUMP_WORDS / world positions drawn from a fixed seed in a range that does not
+    depend on n, so that two builds dump the same positions even when they disagree on n; a position at or past
+    n_words holds -1."""
+    words = d_idx[:n_words].cpu().numpy().view(np.uint32)
+    pos = np.sort(np.random.default_rng(0x5EED1234).choice(DUMP_RANGE, DUMP_WORDS // world, replace=False))
+    vals = np.full(len(pos), -1.0)
+    inside = pos < len(words)
+    vals[inside] = words[pos[inside]]
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, prefix + "stage1_result.npy"), np.array([0, n], dtype=np.float64))  # a failed step raises before this
+    np.save(os.path.join(out_dir, prefix + "structural_indexes.npy"), vals)
+    np.save(os.path.join(out_dir, prefix + "structural_index_positions.npy"), pos.astype(np.float64))
 
 
 # =============================================================================== our arm
@@ -447,6 +471,9 @@ def run_ours(args, rank, world):
     with ClockSampler(local) as clocks:
         total_ms = run_steps(args.steps, True)
     launches2 = parser.get_stat("launches")
+    if args.dump_outputs:
+        n_last = results[(args.steps - 1) % ROTATE][0]
+        dump_outputs(args.dump_outputs, d_idxs[(args.steps - 1) % ROTATE], n_last, n_last + 3 if world == 1 else n_last, world, f"rank{rank}_" if world > 1 else "")
     sharded_host = None
     if world > 1:  # where the host's time went in the timed region (and the warm-up): per rank on stderr, rank 0's in the line
         sharded_host = {"enqueue_ms": round(host_ms["enqueue"], 3), "finish_ms": round(host_ms["finish"], 3), "finish_max_ms": round(host_ms["finish_max"], 3),
@@ -523,7 +550,7 @@ def run_ours(args, rank, world):
             "metric": METRIC, "value": round(value, 2), "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": warmup_steps,
             "ms_per_step": round(ms_per_step, 5), "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u8", "data": "synthetic",
             "config": {"workload": workload_name(world), "bytes_per_gpu_per_step": DOC_BYTES, "mode": "regular" if world == 1 else "shard", "structurals_per_step": int(nmean),
-                       "l2": f"{ROTATE} distinct inputs used round-robin ({ROTATE * DOC_BYTES >> 20} MiB > 126 MB L2)",
+                       "l2": f"{ROTATE} distinct inputs used round-robin ({ROTATE * DOC_BYTES >> 20} MiB > 50 MB L2)",
                        "content": "random sequence of 48 distinct 96 KiB random subtrees per document (corpus.random_json): DRAM behaviour of 64 MiB, 4.6 MB of distinct structure",
                        "api": "sjb200_stage1_dev_batch: the K documents of the timed region are queued back to back on one stream" if world == 1 else
                               "sjb200_stage1_sharded_enqueue / _finish: exchange record stored by the scan kernel into every rank's window over NVLink (CUDA IPC); NCCL only for the handle exchange at start-up"},
@@ -556,7 +583,12 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--config", default="stage1_64m", choices=["stage1_64m", "jsonexamples", "ndjson_1g", "utf8_minify_256m", "concat_8g", "tokens_64m"])
     ap.add_argument("--check", action="store_true", help="parity gate of the multi-rank path on adversarial cuts")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy (default config)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and (args.check or args.config != "stage1_64m" or args.impl != "ours"):
+        ap.error("--dump-outputs applies to the default config of --impl ours")
     rank = int(os.environ.get("RANK", 0))
     world = int(os.environ.get("WORLD_SIZE", 1))
     if args.impl == "reference":

@@ -82,12 +82,9 @@ def run_jsonexamples(args, rank, world):
     rc, parser = sj.get_active_implementation(local).create_dom_parser_implementation(4 << 20)
     parser.set_option("time_kernel", 1)
     files, ok = [], True
-    steps = max(10, args.steps)
+    steps = args.steps
     for name, mode in (("twitter.json", 0), ("citm_catalog.json", 0), ("amazon_cellphones.ndjson", 2)):
-        path = os.path.join(O.JSONEXAMPLES, name)
-        if not os.path.exists(path):
-            continue
-        data = np.fromfile(path, dtype=np.uint8)
+        data = np.frombuffer(O.jsonexample(name), dtype=np.uint8).copy()
         d = torch.from_numpy(data).to(dev)
         want = port.stage1(data, mode)
         for _ in range(3):
@@ -142,7 +139,7 @@ def run_ndjson(args, rank, world, total=1 << 30):
     stream = torch.cuda.Stream(device=dev)
     torch.cuda.set_stream(stream)
     comm = _connect(torch, dist, sharding, parser, rank, world, dev) if world > 1 else None
-    steps = max(3, min(args.steps, 20))
+    steps = args.steps
     last = None
 
     def one_pass():
@@ -185,8 +182,8 @@ def run_ndjson(args, rank, world, total=1 << 30):
     ok = _all_ok(torch, dist, dev, world, bool(ok))
     if rank == 0:
         line = _line(args, world, total / (ms * 1e-3) / 1e9, ms,
-                     {"workload": f"1 GiB NDJSON (amazon_cellphones-style rows), stage1 " + ("streaming_final on 1xB200" if world == 1 else f"sharded after line feeds over {world}xB200") + " (BASELINE.json configs[2])",
-                      "bytes_total": total, "structurals": n, "l2": "1 GiB input >> 126 MB L2",
+                     {"workload": f"1 GiB NDJSON (amazon_cellphones-style rows), stage1 " + ("streaming_final on 1xH100" if world == 1 else f"sharded after line feeds over {world}xH100") + " (BASELINE.json configs[2])",
+                      "bytes_total": total, "structurals": n, "l2": "1 GiB input >> 50 MB L2",
                       "api": "sjb200_stage1_dev" if world == 1 else "sjb200_stage1_sharded (exchange fused into the scan kernel)"},
                      {"parity": {"ok": ok, "against": "CPU oracle on the whole shard of every rank" + (" + 64-bit index bases" if world > 1 else ", (n+3) index words")},
                       "gpu_launches": int(steps), "roofline": _roofline(len(shard) + 4 * (last[1]) + 12, kms, "scan4_kernel"),
@@ -206,7 +203,7 @@ def run_utf8_minify(args, rank, world, size=256 << 20):
     from simdjson_b200 import corpus
     O = B.oracle()
     port = O.Port()
-    steps = max(3, min(args.steps, 20))
+    steps = args.steps
     rc, parser = sj.get_active_implementation(local).create_dom_parser_implementation(size)
     parser.set_option("time_kernel", 1)
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
@@ -220,7 +217,7 @@ def run_utf8_minify(args, rank, world, size=256 << 20):
         ok = ok and parser.validate_utf8_device(bad) == 0
         del bad
     ts = []
-    for it in range(steps):
+    for it in range(steps + 1):  # the first call is not timed
         flush.fill_(it)
         torch.cuda.synchronize()
         parser.validate_utf8_device(du)
@@ -235,7 +232,7 @@ def run_utf8_minify(args, rank, world, size=256 << 20):
     rcm, dl = parser.minify_device(dj, dst)
     okm = rcm == werr and dl == len(wout) and torch.equal(dst[:dl].cpu(), torch.from_numpy(np.frombuffer(wout, dtype=np.uint8).copy()))
     ts = []
-    for it in range(steps):
+    for it in range(steps + 1):
         flush.fill_(it)
         torch.cuda.synchronize()
         parser.minify_device(dj, dst)
@@ -243,9 +240,9 @@ def run_utf8_minify(args, rank, world, size=256 << 20):
     mms = float(np.mean(ts[1:]))
     ok = bool(ok and okm)
     line = _line(args, 1, size / (ums * 1e-3) / 1e9, ums,
-                 {"workload": "validate_utf8 + minify on 256 MiB mixed-ASCII/UTF-8 synthetic, 1xB200 (BASELINE.json configs[3])", "bytes": size,
+                 {"workload": "validate_utf8 + minify on 256 MiB mixed-ASCII/UTF-8 synthetic, 1xH100 (BASELINE.json configs[3])", "bytes": size,
                   "l2": "a 256 MiB buffer is written between launches (cold L2)", "value_is": "validate_utf8 input GB/s (kernel); minify below"},
-                 {"parity": {"ok": ok, "against": "CPU oracle: verdict (valid + 3 corrupted copies), whole minified buffer"}, "gpu_launches": 2 * steps + 5,
+                 {"parity": {"ok": ok, "against": "CPU oracle: verdict (valid + 3 corrupted copies), whole minified buffer"}, "gpu_launches": 2 * (steps + 1) + 5,
                   "roofline": dict(_roofline(size, ums, "utf8v2_kernel"), kernel="sjb200::utf8v2_kernel (sjb200_utf8.cuh)"),
                   "minify": {"input_gbs": round(size / (mms * 1e-3) / 1e9, 1), "kept_fraction": round(dl / size, 4), "kernel_ms": round(mms, 5),
                              "roofline": dict(_roofline(size + dl, mms, "scan4_minify_kernel"), kernel="sjb200::scan4_minify_kernel (1 B read + kept bytes written per input byte)")},
@@ -265,7 +262,7 @@ def run_tokens(args, rank, world, size=64 << 20):
     from simdjson_b200 import corpus
     O = B.oracle()
     port = O.Port()
-    steps = max(3, min(args.steps, 20))
+    steps = args.steps
     doc = corpus.random_json(size).copy()
     d = torch.from_numpy(doc).to(dev)
     rc, parser = sj.get_active_implementation(local).create_dom_parser_implementation(size)
@@ -301,7 +298,7 @@ def run_tokens(args, rank, world, size=64 << 20):
     # algorithmic bytes: the document once + the index array in, type + payload + string buffer out
     algo = size + 4 * n + 9 * n + int(res.string_bytes)
     line = _line(args, 1, size / (ms * 1e-3) / 1e9, ms,
-                 {"workload": "stage-2-lite (token types, integer values, string buffer) on the synthetic 64 MiB document of BASELINE.json configs[1], 1xB200 (SURVEY.md 8(f) row 4)",
+                 {"workload": "stage-2-lite (token types, integer values, string buffer) on the synthetic 64 MiB document of BASELINE.json configs[1], 1xH100 (SURVEY.md 8(f) row 4)",
                   "bytes": size, "structurals": int(n), "strings": int(res.n_strings), "string_buf_bytes": int(res.string_bytes),
                   "l2": "a 256 MiB buffer is written between calls (cold L2)", "value_is": "document bytes per second through sjb200_tokens_dev (3 launches + the 24-byte result)",
                   "api": "sjb200_tokens_dev", "tok_stage": int(os.environ.get("SJB200_TOK_STAGE", "1"))},
@@ -323,7 +320,7 @@ def run_concat(args, rank, world, nshards=8, shard_target=1 << 30):
     port = O.Port()
     if nshards % world != 0:
         raise SystemExit("concat_8g needs 1, 2, 4 or 8 ranks")
-    unit = b"".join(open(os.path.join(O.JSONEXAMPLES, f), "rb").read() + b"\n" for f in ("twitter.json", "citm_catalog.json"))
+    unit = b"".join(O.jsonexample(f) + b"\n" for f in ("twitter.json", "citm_catalog.json"))
     unit_a = np.frombuffer(unit, dtype=np.uint8)
     reps = shard_target // len(unit)
     shard = np.tile(unit_a, reps)  # every shard is the same bytes: reps whole (twitter, citm) pairs, cut at a document boundary
@@ -337,7 +334,7 @@ def run_concat(args, rank, world, nshards=8, shard_target=1 << 30):
     torch.cuda.set_stream(stream)
     comm = _connect(torch, dist, sharding, parser, rank, world, dev) if world > 1 else sharding.Comm(parser, 0, 1)
     rounds = nshards // world
-    steps = max(2, min(args.steps, 5))
+    steps = args.steps
 
     def whole_job():
         """8 shards: `rounds` sharded passes of `world` shards each; 64-bit bases accumulate over the rounds on the host"""
@@ -375,7 +372,7 @@ def run_concat(args, rank, world, nshards=8, shard_target=1 << 30):
     if rank == 0:
         nbytes = nshards * len(shard)
         line = _line(args, world, nbytes / (ms * 1e-3) / 1e9, ms,
-                     {"workload": f"8 GB concatenated jsonexamples corpus (twitter/citm_catalog repeated), stage1 sharded across {world}xB200 with carry fixup (BASELINE.json configs[4])",
+                     {"workload": f"8 GB concatenated jsonexamples corpus (twitter/citm_catalog repeated), stage1 sharded across {world}xH100 with carry fixup (BASELINE.json configs[4])",
                       "bytes_total": int(nbytes), "shards": nshards, "shard_bytes": int(len(shard)), "passes_per_job": rounds, "structurals_total": int(total),
                       "bases": "64-bit: shard-relative uint32 indexes + uint64 base per shard (document_stream-inl.h L250)",
                       "api": "sjb200_stage1_sharded: exchange record stored by the scan kernel into every rank's window (CUDA IPC over NVLink)"},

@@ -1,5 +1,5 @@
 /*
- * sjb200.h -- C ABI of the B200 (sm_100a) stage-1 / minify / validate_utf8 library.
+ * sjb200.h -- C ABI of the H100 (sm_90a) stage-1 / minify / validate_utf8 library.
  *
  * This is the drop-in boundary for ONE hot path of simdjson (SURVEY.md section 8): it exports exactly
  * what a `simdjson::implementation` / `internal::dom_parser_implementation` back-end has to provide

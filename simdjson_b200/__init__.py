@@ -1,5 +1,5 @@
 """simdjson_b200 -- simdjson's stage 1 (structural indexing + UTF-8 validation), minify and
-validate_utf8 as hand-written sm_100a CUDA kernels behind simdjson's own plug-in boundary.
+validate_utf8 as hand-written sm_90a CUDA kernels behind simdjson's own plug-in boundary.
 
   csrc/            CUDA kernels + the C ABI (include/sjb200.h) -> libsjb200.so
   plugin/          C++ shim: simdjson::implementation / dom_parser_implementation subclasses ("b200")

@@ -55,7 +55,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a).  simdjson_b200 has no CPU fallback.")
+            "(nvcc, sm_90a).  simdjson_b200 has no CPU fallback.")
     L = C.CDLL(LIB_PATH)
     u8p, u32p, vp, sz = C.POINTER(C.c_uint8), C.POINTER(C.c_uint32), C.c_void_p, C.c_size_t
     sig = {

@@ -1,4 +1,4 @@
-// sjb200_bits.cuh -- the per-lane bit-plane arithmetic of the B200 stage-1 kernels.
+// sjb200_bits.cuh -- the per-lane bit-plane arithmetic of the H100 stage-1 kernels.
 //
 // Everything in this header is a pure function of its arguments (no warp
 // intrinsics, no memory), compiled for both host and device, so that the
@@ -73,7 +73,7 @@ SJ_HD uint32_t bitsel(uint32_t m, uint32_t a, uint32_t b) {
 
 // x >> d for a constant d, on the FMA pipe (IMAD.HI) instead of the ALU pipe (SHF): the scan is bound by the ALU pipe's
 // issue rate, the FMA pipe is mostly idle.  Build option; the multiply is slower per instruction, so it only pays if
-// it overlaps (measured per build in profiles/).
+// it overlaps (compare the two builds).
 #ifndef SJB200_SHR_IMAD
 #define SJB200_SHR_IMAD 0
 #endif

@@ -92,7 +92,8 @@ struct sjb200_ctx {
   std::vector<cudaEvent_t> ring_events;
   CopyPool *pool = nullptr;
   long opt_force_grid = 0;
-  long opt_ew_min_bytes = 384l << 20;  // stage-1 launches of at least this many bytes run the emit-warp build of the kernel (0: never)
+  long opt_ew_min_bytes = 0;  // stage-1 launches of at least this many bytes run the emit-warp build of the kernel (0: never, the
+                              // default: on H100 that build was slower at every launch size from 256 MiB to 1 GiB)
   long opt_host_skip_scan = 0;  // tuning: the host-pointer pipeline copies only (no scan launches; results are meaningless)
   long opt_copy_threads = 4;        // 0: no staging (cudaMemcpyAsync straight from the caller's memory)
   long opt_ring_slots = 8;
@@ -333,9 +334,9 @@ extern "C" int sjb200_create(int device, size_t capacity, sjb200_ctx **out) {
     return SJB200_UNSUPPORTED_ARCHITECTURE;
   }
   cudaDeviceProp prop;
-  if (cudaGetDeviceProperties(&prop, device) != cudaSuccess || prop.major != 10) {
+  if (cudaGetDeviceProperties(&prop, device) != cudaSuccess || prop.major != 9 || prop.minor != 0) {
     (void)cudaGetLastError();
-    return SJB200_UNSUPPORTED_ARCHITECTURE;  // the kernel image is sm_100a only
+    return SJB200_UNSUPPORTED_ARCHITECTURE;  // the kernel image is sm_90a only
   }
   sjb200_ctx *c = new (std::nothrow) sjb200_ctx();
   if (!c) return SJB200_MEMALLOC;

@@ -1,7 +1,7 @@
 // sjb200_hostcopy.cpp -- the copy loop of the staging threads (sjb200_hostpipe.h): pageable source -> page-locked ring.
 // Streaming (non-temporal) stores: the destination is about to be read by the copy engine, not by this core, and a
 // plain memcpy of a sub-megabyte piece first READS every destination line (write-allocate), which halves what a thread
-// moves (measured on the bench box: ~8 GB/s per thread with memcpy in 1 MiB pieces, ~16 GB/s streaming).
+// moves.
 #include <stddef.h>
 #include <stdint.h>
 #include <string.h>

@@ -5,7 +5,7 @@
 // cudaMemcpyAsync from pageable memory is staged by the driver one piece at a time and blocks the calling thread, which
 // leaves most of the PCIe link idle; page-locking the caller's buffer per call costs more than the copy, and keeping it
 // locked after the call is not safe (the caller may free and re-map the range).  So the library owns a fixed ring of
-// page-locked slots and fills it with plain memcpy from several threads (one core moves ~10 GB/s, the link ~55 GB/s),
+// page-locked slots and fills it with plain memcpy from several threads (one core cannot fill the link),
 // while the copy engine drains the slots and the scan kernels chase the copies (document_stream gets its overlap from a
 // worker thread in the same spirit: include/simdjson/dom/document_stream-inl.h L16-85, L321-344).
 //

@@ -1,4 +1,4 @@
-// sjb200_kernels.cu -- the sm_100a kernels' entry points and launchers.
+// sjb200_kernels.cu -- the sm_90a kernels' entry points and launchers.
 //
 // What the kernels replace in the reference (CPU, 64-byte SIMD blocks, strictly serial carries):
 //   json_structural_indexer::index<128> / step / next   src/generic/stage1/json_structural_indexer.h L193-247

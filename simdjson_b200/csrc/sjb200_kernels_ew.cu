@@ -1,11 +1,12 @@
-// sjb200_kernels_ew.cu -- the emit-warp build of the stage-1 kernel (same source: sjb200_scan4.cuh), for large launches.
+// sjb200_kernels_ew.cu -- the emit-warp build of the stage-1 kernel (same source: sjb200_scan4.cuh), an option for large launches.
 //
 // Default build (sjb200_kernels.cu): a scan warp emits the block it scanned two iterations earlier (masks wait in shared
 // memory).  This build: the 16 scan warps only scan, 7 more warps per CTA take resolved blocks from a CTA-wide queue
 // and emit them; the masks wait in an L2-resident ring 8 elements deep, so a scan warp never waits for the chain.
-// Measured on B200 (profiles/README.md): break-even at 256 MiB per launch, +3.5 % at 512 MiB, +4.7 % at 1 GiB; slower
-// below (the ring fills before the first element is resolved, and at the end of a short launch only the emit is left to
-// do): the host code picks this kernel for launches of at least `ew_min_bytes` (option; 384 MiB).
+// It pays off only for large launches (below, the ring fills before the first element is resolved, and at the end of a
+// short launch only the emit is left to do): the host code picks this kernel for launches of at least `ew_min_bytes`
+// (option; 0 = never, the default: on H100 this build was slower than the default one at every launch size from
+// 256 MiB to 1 GiB, 13-16 % on NDJSON).
 #ifdef SJB200_SCAN4_EMITW
 #undef SJB200_SCAN4_EMITW
 #endif

@@ -8,7 +8,7 @@
 //   bit_indexer::write                                   json_structural_indexer.h L93-122 (src/icelake.cpp L129-160)
 //   utf8_checker                                         utf8_lookup4_algorithm.h L145-202
 //
-// Design (B200-first; nothing here resembles the reference's block loop):
+// Design (GPU-first; nothing here resembles the reference's block loop):
 //   * The document is cut into 4 KiB *blocks* (one TMA box of 32 rows x 128 B, 128B-swizzled, so lane L owns row L and
 //     reads it with conflict-free LDS.128) and *elements* of kScanWarps consecutive blocks (64 KiB), one block per scan warp.
 //   * A CTA is kScanWarps (16) independent *scan warps* + 1 *chain warp*, persistent, one CTA per SM, pulling elements
@@ -41,9 +41,8 @@ namespace scan4 {
 #ifndef SJB200_SCAN4_WARPS
 #define SJB200_SCAN4_WARPS 16
 #endif
-constexpr int kScanWarps = SJB200_SCAN4_WARPS;  // scan warps per CTA = blocks per element.  16 (one CTA per SM, 64 KiB elements) measured
-                                                // 10 % faster at 64 MiB and 25 % faster at 1 GiB than 8 (two CTAs per SM): half the chain warps
-                                                // polling the descriptors, half the elements to resolve
+constexpr int kScanWarps = SJB200_SCAN4_WARPS;  // scan warps per CTA = blocks per element.  16 (one CTA per SM, 64 KiB elements) rather than
+                                                // 8 (two CTAs per SM): half the chain warps polling the descriptors, half the elements to resolve
 constexpr int kBlockBytes = 4096;
 constexpr int kBlockRows = kBlockBytes / 128;
 constexpr int kChainWarps = 1;  // the warp that resolves this CTA's elements
@@ -51,8 +50,8 @@ constexpr int kChainWarps = 1;  // the warp that resolves this CTA's elements
 #define SJB200_SCAN4_EMITW 0
 #endif
 // Emit warps (stage 1 only): the scan is bound by the ALU pipe, the emit by FLO / shared-memory latency.  When the warp
-// that scanned a block also emits it, all warps of the CTA sit in the emit loop together (measured: ~2300 of the ~9200
-// cycles of an iteration with the ALU pipe nearly idle).  Dedicated warps take resolved blocks from a CTA-wide queue
+// that scanned a block also emits it, all warps of the CTA sit in the emit loop together, with the ALU pipe
+// nearly idle.  Dedicated warps take resolved blocks from a CTA-wide queue
 // and emit them while the scan warps go on scanning.  0: every scan warp emits its own blocks (minify always does).
 constexpr int kEmitWarps = SJB200_SCAN4_EMITW;
 constexpr int kThreads4 = 32 * (kScanWarps + kChainWarps + kEmitWarps);
@@ -157,7 +156,7 @@ SJ_DEV Eff compose(const Eff &o, const Eff &n) {
 }
 
 // A waiting warp must not spin at full speed: mbarrier.try_wait returns at once, and a busy loop takes issue slots
-// from the warps that do the work (measured: 20 % of all issued instructions).  `ns` = back-off between polls.
+// from the warps that do the work.  `ns` = back-off between polls.
 #ifndef SJB200_SCAN4_POLL_SCALE
 #define SJB200_SCAN4_POLL_SCALE 1
 #endif
@@ -747,7 +746,7 @@ SJ_DEV bool issue_load(Smem *S, const sj_tensor_map *tmap, const ScanParams &p, 
       sj_mbar_arrive_expect_tx(&S->full[warp][r], kBlockBytes);
       sj_tma_load_rows(S->ring[warp][r], tmap, &S->full[warp][r], uint32_t(row));
     }
-    // after the TMA is on its way: the fence above would otherwise sit out this load's round trip to L2 (measured: ~550 cycles)
+    // after the TMA is on its way: the fence above would otherwise sit out this load's round trip to L2
     *pw_out = (bstart < p.len) ? word_before(p, bstart) : 0x20202020u;
   }
   return full;
@@ -770,8 +769,8 @@ SJ_DEV void scan_role(Smem *S, const sj_tensor_map *tmap, const ScanParams &p, c
   uint32_t pw_cur = 0x20202020u, pw_next = 0x20202020u;
   bool tma_cur = false, tma_next = false;
   // Tickets must not depend on the chain warp's progress (it may sit in a look-back while the scan warps run ahead),
-  // and nobody should wait for a ticket at the top of an iteration (measured with the trace build: with the ticket
-  // published after warp 0's scan, every other warp waited ~1100 cycles per iteration): the ticket of element j + 2 is
+  // and nobody should wait for a ticket at the top of an iteration (with the ticket published after warp 0's scan,
+  // every other warp waited for it in every iteration): the ticket of element j + 2 is
   // drawn and published at the top of iteration j, it is needed at the top of iteration j + 1.
   // Tickets should be scanned in roughly the order they were taken (every element waits for ALL lower tickets): at
   // start-up the second ticket is therefore taken only once the first block has arrived, when every CTA of the launch
@@ -794,7 +793,7 @@ SJ_DEV void scan_role(Smem *S, const sj_tensor_map *tmap, const ScanParams &p, c
     SJ_TRACE4(0);
     const uint32_t tn = wait_ticket(S, j + 1, p);
     if (warp == (j % uint32_t(kScanWarps))) {
-      // ticket duty rotates: this warp draws the CTA's element j + 2 and waits for the atomic's round trip (~700 cycles)
+      // ticket duty rotates: this warp draws the CTA's element j + 2 and waits for the atomic's round trip
       // before it goes on; the others need that ticket one iteration from now.  (A ticket is scanned two iterations after
       // it was drawn -- every element of the launch waits for ALL lower tickets, so tickets should not be held longer
       // than the TMA pipeline needs -- and no warp is always the one that pays for the round trip.)  Drawn only after
@@ -1111,8 +1110,8 @@ SJ_DEV void chain_role(Smem *S, const ScanParams &p, const Carry &cin, unsigned 
     if (t >= nelem) break;
     uint32_t s_in = (cin.state >> 1) & 1u, base = 0;
     // The look-back needs the elements BEFORE t, not t itself: it runs while this CTA is still scanning t, so that the
-    // element is resolved as soon as its own summary is there (with the look-back after the scan, an element was
-    // resolved ~3.6 us after the last of its predecessors had been scanned: pick-up + poll round trips + fold).
+    // element is resolved as soon as its own summary is there (with the look-back after the scan, an element waited
+    // after the last of its predecessors had been scanned for the pick-up, the poll round trips and the fold).
     if (t > 0) look_back(p, t, lane, &s_in, &base);
     wait_bar(&S->scanned[ns], (j / kNS) & 1u, p, 64);
     if (!SJB200_SCAN4_TRACE && p.debug != nullptr && lane == 0) p.debug[uint64_t(t) * 8 + 6] = sj_globaltimer();
@@ -1154,7 +1153,7 @@ SJ_DEV void scan4_body(const sj_tensor_map *tmap, const ScanParams &p, uint8_t *
   Carry cin;
   cin.count = 0; cin.state = 0; cin.ttable = 0; cin.flags = 0; cin.reserved = 0;
   if (p.carry_in != nullptr) cin = *p.carry_in;
-  // ~140 mbarriers: one thread each (a single thread took 1.3 us over them)
+  // ~140 mbarriers: one thread each (a single thread initialising them all is slow)
   if (tid < unsigned(kNS)) {
     sj_mbar_init(&S->ticket_ready[tid], 1);
     sj_mbar_init(&S->scanned[tid], 1);

@@ -1,7 +1,7 @@
 // sjb200_simt.cuh -- the few hardware primitives the scan4 kernel is written against.
 //
 // Two implementations of the same small API:
-//   * nvcc / sm_100a: warp intrinsics, mbarrier + cp.async.bulk.tensor (TMA) inline PTX, relaxed
+//   * nvcc / sm_90a: warp intrinsics, mbarrier + cp.async.bulk.tensor (TMA) inline PTX, relaxed
 //     gpu-scope loads/stores for the look-back descriptors;
 //   * SJB200_HOST_EMU (g++, tests/simt_emul.cpp): one OS thread per CUDA thread, warp collectives as
 //     32-thread rendezvous, mbarriers with deferred TMA copies.  This exists so that the *actual*
@@ -223,7 +223,7 @@ SJ_DEV void sj_tma_load_rows(uint8_t *dst, const sj_tensor_map *map, sj_mbar_t *
 }  // namespace sjb200
 
 #else
-// =============================================================================== sm_100a
+// =============================================================================== sm_90a
 #include <cuda.h>
 #include <cuda_runtime.h>
 
@@ -322,7 +322,7 @@ SJ_DEV void sj_mbar_init(sj_mbar_t *bar, uint32_t count) {
 }
 SJ_DEV void sj_fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 // (MEMBAR.ALL.CTA + FENCE.VIEW.ASYNC: waits for the thread's outstanding loads -- issue it before, not after, a global
-// load whose value is not needed yet.  Measured: a build without it is not faster, profiles/README.md)
+// load whose value is not needed yet)
 SJ_DEV void sj_fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 SJ_DEV void sj_mbar_arrive(sj_mbar_t *bar) {
   asm volatile("mbarrier.arrive.release.cta.shared::cta.b64 _, [%0];" ::"r"(sj_smem_u32(bar)) : "memory");

@@ -6,9 +6,8 @@
 // UTF-8 validity needs no scan: byte i is judged from bytes i-3..i (SURVEY.md 8(a) equivalence note).  So this kernel has
 // no chain, no tickets and no CTA-wide barrier: warp g of the launch takes blocks g, g + G, g + 2G, ... (neighbouring
 // warps read neighbouring 4 KiB blocks), each through its own TMA ring (cp.async.bulk.tensor, 32 rows x 128 B, 128B-swizzled:
-// lane L owns row L and reads it with conflict-free LDS.128; kSlotsU slots, kSlotsU - 1 blocks in flight).  Measured
-// (profiles/README.md): 24 warps x 2 slots per SM beat 18 x 3, 13 x 4 and 10 x 5 -- ASCII and multi-byte text take the
-// same time, the kernel streams at ~4.8 TB/s whatever the ring depth.  One
+// lane L owns row L and reads it with conflict-free LDS.128; kSlotsU slots, kSlotsU - 1 blocks in flight; 24 warps x 2
+// slots per SM).  One
 // vote per block: without a byte >= 0x80 in any lane a block costs ~50 instructions; otherwise the lane's four 32-byte
 // units are transposed into bit planes and checked with the boolean rules of sjb200_bits.cuh, without further votes.
 // The three bytes before a lane's row come from the row before it (shared memory), those before a block from global

@@ -239,7 +239,7 @@ class dom_parser_implementation:
 
 
 class implementation:
-    """simdjson::implementation for the B200 (include/simdjson/implementation.h L45-160)."""
+    """simdjson::implementation for the H100 (include/simdjson/implementation.h L45-160)."""
 
     def __init__(self, device=0):
         self._device = device
@@ -249,7 +249,7 @@ class implementation:
         return "b200"
 
     def description(self):
-        return "NVIDIA B200 (sm_100a) stage 1"
+        return "NVIDIA H100 (sm_90a) stage 1"
 
     def required_instruction_sets(self):
         return 0

@@ -15,7 +15,7 @@
 // Install (doc/implementation-selection.md L93-110):
 //     simdjson::get_active_implementation() = simdjson::b200::get_implementation();
 // after which dom::parser::parse / parse_many, ondemand::parser::iterate, simdjson::minify and
-// simdjson::validate_utf8 run their stage 1 on the B200.
+// simdjson::validate_utf8 run their stage 1 on the H100.
 #ifndef SIMDJSON_B200_IMPLEMENTATION_H
 #define SIMDJSON_B200_IMPLEMENTATION_H
 
@@ -31,7 +31,7 @@ namespace b200 {
 class implementation final : public simdjson::implementation {
  public:
   explicit implementation(int device = 0)
-      : simdjson::implementation("b200", "NVIDIA B200 (sm_100a) stage 1", /*required_instruction_sets=*/0), device_(device) {}
+      : simdjson::implementation("b200", "NVIDIA H100 (sm_90a) stage 1", /*required_instruction_sets=*/0), device_(device) {}
   simdjson_warn_unused error_code create_dom_parser_implementation(size_t capacity, size_t max_depth,
                                                                    std::unique_ptr<internal::dom_parser_implementation> &dst) const noexcept final;
   simdjson_warn_unused error_code minify(const uint8_t *buf, size_t len, uint8_t *dst, size_t &dst_len) const noexcept final;

@@ -1,10 +1,13 @@
 """ctypes bindings for the two CPU checkers under oracle/ (test infrastructure only).
 
   port : oracle/libsj_oracle.so    -- our byte-at-a-time C restatement (always built)
-  ref  : oracle/_ref/libsj_ref.so  -- the unmodified reference compiled from
-                                      /root/reference/singleheader (may be absent)
+  ref  : oracle/_ref/libsj_ref.so  -- the unmodified reference compiled from its
+                                      singleheader sources by oracle/Makefile (may be absent)
+
+jsonexample(name): the reference's own example corpora, stored xz-compressed under tests/golden/jsonexamples/.
 """
 import ctypes as C
+import lzma
 import os
 import subprocess
 
@@ -14,7 +17,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 ORACLE_DIR = os.path.join(ROOT, "oracle")
 PORT_SO = os.path.join(ORACLE_DIR, "libsj_oracle.so")
 REF_SO = os.path.join(ORACLE_DIR, "_ref", "libsj_ref.so")
-JSONEXAMPLES = os.path.join(ORACLE_DIR, "_ref", "jsonexamples")
+JSONEXAMPLES = os.path.join(ROOT, "tests", "golden", "jsonexamples")
 
 SUCCESS, CAPACITY, MEMALLOC, UTF8_ERROR, EMPTY, UNESCAPED_CHARS, UNCLOSED_STRING, UNEXPECTED_ERROR = 0, 1, 2, 11, 13, 14, 15, 24
 REGULAR, STREAMING_PARTIAL, STREAMING_FINAL, JSON_SEQUENCE_PARTIAL, JSON_SEQUENCE_FINAL, COMMA_DELIMITED_PARTIAL, COMMA_DELIMITED_FINAL = range(7)
@@ -227,6 +230,12 @@ class Ref:
         fe = C.c_int(0)
         nd = self.L.sjr_dom_parse_many(self.impl, _ptr(a), len(a), batch_size, out, cap, C.byref(ol), C.byref(fe))
         return nd, fe.value, out.raw[: ol.value]
+
+
+def jsonexample(name):
+    """the bytes of one of the reference's corpora (twitter.json, citm_catalog.json, amazon_cellphones.ndjson)"""
+    with lzma.open(os.path.join(JSONEXAMPLES, name + ".xz")) as f:
+        return f.read()
 
 
 def have_ref():

@@ -46,7 +46,7 @@ def test_pure_host_helpers():
 
 
 def test_no_cpu_fallback_without_gpu():
-    """Without a usable sm_100 device the product must fail loudly, not fall back."""
+    """Without a usable sm_90 device the product must fail loudly, not fall back."""
     import torch
     if torch.cuda.is_available():
         return

@@ -58,10 +58,9 @@ def test_port_matches_golden_utf8(port):
         assert port.validate_utf8(bytes.fromhex(c["hex"])) == c["valid"], c
 
 
-@pytest.mark.skipif(not os.path.isdir(O.JSONEXAMPLES), reason="reference corpora not staged (make -C oracle)")
 def test_port_matches_golden_corpora(port):
     for f in _load("corpora.json")["files"]:
-        data = np.fromfile(os.path.join(O.JSONEXAMPLES, f["file"]), dtype=np.uint8)
+        data = np.frombuffer(O.jsonexample(f["file"]), dtype=np.uint8)
         assert len(data) == f["len"]
         r = port.stage1(data, f["mode"])
         assert (r.err, r.n) == (f["err"], f["n"])
@@ -74,10 +73,7 @@ def test_port_matches_golden_corpora(port):
 def test_amazon_is_793_documents(port):
     """tests/dom/basictests.cpp L36, L692-708: parse_many over amazon_cellphones.ndjson yields 793 docs;
     at stage-1 level: 793 top-level '[' ... ']' rows in streaming_final mode."""
-    path = os.path.join(O.JSONEXAMPLES, "amazon_cellphones.ndjson")
-    if not os.path.exists(path):
-        pytest.skip("reference corpora not staged")
-    data = np.fromfile(path, dtype=np.uint8)
+    data = np.frombuffer(O.jsonexample("amazon_cellphones.ndjson"), dtype=np.uint8)
     r = port.stage1(data, O.STREAMING_FINAL)
     assert r.err == 0 and r.n == 15067
     # count row starts: a '[' structural that is the first structural on its line
@@ -203,7 +199,7 @@ def test_port_tokens_match_golden(port):
     for c in g["documents"]:
         _check_doc_against(port, bytes.fromhex(c["doc"]), c["err"], c["types"].encode("latin1"), c["payloads"], bytes.fromhex(c["string_buf"]))
     for f in g["files"]:
-        doc = open(os.path.join(O.JSONEXAMPLES, f["file"]), "rb").read()
+        doc = O.jsonexample(f["file"])
         r = port.stage1(doc)
         err, types, pay, sb, sl, ns, fe = port.tokens(doc, r.idx, r.n)
         t, p = _tape_view(types, pay)

@@ -3,7 +3,7 @@
 set -e
 cd "$(dirname "$0")/.."
 SRCS="simdjson_b200/csrc/sjb200_kernels.cu simdjson_b200/csrc/sjb200_kernels_ew.cu simdjson_b200/csrc/sjb200_docs.cu simdjson_b200/csrc/sjb200_capi.cu simdjson_b200/csrc/sjb200_finish.cpp simdjson_b200/csrc/sjb200_hostcopy.cpp"
-FLAGS="-O3 -std=c++17 -lineinfo -gencode arch=compute_100a,code=sm_100a -Xcompiler -fPIC,-fvisibility=hidden -shared"
+FLAGS="-O3 -std=c++17 -lineinfo -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fvisibility=hidden -shared"
 mkdir -p tools/variants
 rm -f tools/variants/*.so
 build() { name=$1; shift; nvcc $FLAGS "$@" -o tools/variants/lib_$name.so $SRCS & }

@@ -1,4 +1,4 @@
-// microbench.cu -- integer pipe throughput on sm_100a (SURVEY.md section 7, hard part 1:
+// microbench.cu -- integer pipe throughput on sm_90a (SURVEY.md section 7, hard part 1:
 // "measure LOP3/PRMT/IADD3/IMAD throughput on the box before designing").
 // Prints lane-ops per clock per SM for a few instruction mixes.  Diagnostic tool only.
 #include <cuda_runtime.h>

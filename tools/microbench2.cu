@@ -1,4 +1,4 @@
-// microbench2.cu -- exact-instruction integer pipe probes for sm_100a (inline PTX so the compiler cannot re-associate):
+// microbench2.cu -- exact-instruction integer pipe probes for sm_90a (inline PTX so the compiler cannot re-associate):
 // is IMAD.HI (a right shift on the FMA pipe) full rate?  how do the delta-swap formulations compare?  Diagnostic only.
 #include <cuda_runtime.h>
 #include <stdint.h>

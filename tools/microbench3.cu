@@ -3,7 +3,7 @@
 //   2. copy engine: pinned H2D, D2H, both at once; H2D from pageable memory
 //   3. kernel stores to mapped host memory
 //   4. memcpy pageable -> pinned with T threads
-// build: nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o tools/microbench3 tools/microbench3.cu -lpthread
+// build: nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o tools/microbench3 tools/microbench3.cu -lpthread
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -50,14 +50,14 @@ int main() {
   cudaFuncSetAttribute(k_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
   printf("== empty kernels, event to event\n");
   printf("<<<1,32>>>                 : "); time_launch(s, 20, [](cudaStream_t st) { k_empty<<<1, 32, 0, st>>>(g_flag); }); printf("\n");
-  printf("<<<148,544>>>              : "); time_launch(s, 20, [](cudaStream_t st) { k_empty<<<148, 544, 0, st>>>(g_flag); }); printf("\n");
-  printf("<<<148,544>>> 128 B param  : "); time_launch(s, 20, [](cudaStream_t st) { Big b; memset(&b, 1, sizeof(b)); k_empty_big<<<148, 544, 0, st>>>(b, g_flag); }); printf("\n");
-  printf("<<<148,544, 64 KB>>>       : "); time_launch(s, 20, [](cudaStream_t st) { k_smem<<<148, 544, 64 * 1024, st>>>(g_flag); }); printf("\n");
-  printf("<<<148,544, 199 KB>>>      : "); time_launch(s, 20, [](cudaStream_t st) { k_smem<<<148, 544, 199 * 1024, st>>>(g_flag); }); printf("\n");
-  printf("<<<148,544, 199 KB>>> x2 (two back to back between the events): ");
-  time_launch(s, 20, [](cudaStream_t st) { k_smem<<<148, 544, 199 * 1024, st>>>(g_flag); k_smem<<<148, 544, 199 * 1024, st>>>(g_flag); }); printf("\n");
-  printf("<<<148,544,199 KB>>> after <<<.., 0 KB>>> (carve-out switch): ");
-  time_launch(s, 20, [](cudaStream_t st) { k_empty<<<148, 544, 0, st>>>(g_flag); k_smem<<<148, 544, 199 * 1024, st>>>(g_flag); }); printf("\n");
+  printf("<<<132,544>>>              : "); time_launch(s, 20, [](cudaStream_t st) { k_empty<<<132, 544, 0, st>>>(g_flag); }); printf("\n");
+  printf("<<<132,544>>> 128 B param  : "); time_launch(s, 20, [](cudaStream_t st) { Big b; memset(&b, 1, sizeof(b)); k_empty_big<<<132, 544, 0, st>>>(b, g_flag); }); printf("\n");
+  printf("<<<132,544, 64 KB>>>       : "); time_launch(s, 20, [](cudaStream_t st) { k_smem<<<132, 544, 64 * 1024, st>>>(g_flag); }); printf("\n");
+  printf("<<<132,544, 199 KB>>>      : "); time_launch(s, 20, [](cudaStream_t st) { k_smem<<<132, 544, 199 * 1024, st>>>(g_flag); }); printf("\n");
+  printf("<<<132,544, 199 KB>>> x2 (two back to back between the events): ");
+  time_launch(s, 20, [](cudaStream_t st) { k_smem<<<132, 544, 199 * 1024, st>>>(g_flag); k_smem<<<132, 544, 199 * 1024, st>>>(g_flag); }); printf("\n");
+  printf("<<<132,544,199 KB>>> after <<<.., 0 KB>>> (carve-out switch): ");
+  time_launch(s, 20, [](cudaStream_t st) { k_empty<<<132, 544, 0, st>>>(g_flag); k_smem<<<132, 544, 199 * 1024, st>>>(g_flag); }); printf("\n");
   printf("events only                : "); time_launch(s, 20, [](cudaStream_t) {}); printf("\n");
 
   const size_t N = 64u << 20, M = 24u << 20;
@@ -85,7 +85,7 @@ int main() {
   printf("== kernel stores to mapped host memory (24 MiB, 16-byte vectors)\n");
   uint4 *hq_dev = nullptr;
   cudaHostGetDevicePointer((void **)&hq_dev, hq, 0);
-  for (int grid : {8, 32, 148}) {
+  for (int grid : {8, 32, 132}) {
     double t = wall([&] { k_store_host<<<grid, 256, 0, s>>>(hq_dev, M / 16); cudaStreamSynchronize(s); });
     t = wall([&] { k_store_host<<<grid, 256, 0, s>>>(hq_dev, M / 16); cudaStreamSynchronize(s); });
     printf("grid %3d: %.1f GB/s | ", grid, M / t / 1e9);

@@ -1,5 +1,5 @@
-"""Summarise one `ncu --set full` report into the JSON kept under profiles/ (the .ncu-rep itself stays in gpurun_out/).
-usage: python tools/ncu_summary.py gpurun_out/scan4_full.ncu-rep profiles/NAME.json"""
+"""Summarise one `ncu --set full` report into a small JSON file (kernel name, DRAM bytes, the kernel sources' hash).
+usage: python tools/ncu_summary.py REPORT.ncu-rep OUT.json"""
 import csv
 import hashlib
 import json

@@ -13,6 +13,9 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 import simdjson_b200 as sj  # noqa: E402
 from simdjson_b200 import corpus  # noqa: E402
+from bench import peaks  # noqa: E402
+
+PEAK_GBS = peaks()[0]  # MEASURED_PEAKS.json hbm_gbs, else the data sheet's figure
 
 size = int(os.environ.get("PROBE_BYTES", 64 << 20))
 tag = os.environ.get("PROBE_TAG") or os.path.basename(os.environ.get("SJB200_LIB", "default"))
@@ -54,7 +57,7 @@ for it in range(6):
     cold.append(p.get_stat("kernel_ms"))
 alg = size + 4 * want_n + 12
 res.update({"warm_ms": min(warm[2:]), "cold_ms": min(cold[1:]), "cold_med_ms": sorted(cold[1:])[len(cold[1:]) // 2],
-            "in_gbs_cold": size / min(cold[1:]) / 1e6, "alg_frac_cold": alg / min(cold[1:]) / 1e6 / 6583.5})
+            "in_gbs_cold": size / min(cold[1:]) / 1e6, "alg_frac_cold": alg / min(cold[1:]) / 1e6 / PEAK_GBS})
 print(json.dumps(res), flush=True)
 os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
 with open(os.path.join(ROOT, "gpurun_out", "probe2.jsonl"), "a") as f:

@@ -5,6 +5,7 @@ import os
 import sys
 
 import numpy as np
+import pynvml
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -27,7 +28,7 @@ n = sj.lib().sjb200_get_debug_timeline(p._ctx, buf.ctypes.data, rows)
 IT, PTS = 8, 12
 names = ["top", "ticket", "load issued", "data here", "boundary", "scanned", "arrive/compose", "publish", "resolved seen", "emitted"]
 ctas = []
-for c in range(148):
+for c in range(torch.cuda.get_device_properties(0).multi_processor_count):  # one CTA per SM
     r = buf[c * (1 + 2 * IT): (c + 1) * (1 + 2 * IT)]
     if r[0, 0] == 0:
         continue
@@ -46,9 +47,10 @@ t_exit = np.array([c[1][3] for c in ctas], dtype=np.int64)
 t0 = t_entry.min()
 print(f"kernel_ms (events) {kms:.4f}; CTAs {len(ctas)}")
 print(f"CTA entry: first 0.00, last {(t_entry.max()-t0)/1e3:.2f} us; roles start mean {(t_roles-t0).mean()/1e3:.2f}; scan role done mean {(t_done-t0).mean()/1e3:.2f} max {(t_done.max()-t0)/1e3:.2f}; exit max {(t_exit.max()-t0)/1e3:.2f} us")
-clk = 1.965e3  # cycles per us (nominal)
+pynvml.nvmlInit()
+clk = float(pynvml.nvmlDeviceGetMaxClockInfo(pynvml.nvmlDeviceGetHandleByIndex(torch.cuda.current_device()), pynvml.NVML_CLOCK_SM))  # cycles per us
 for a, wname in ((0, "warp 0"), (1, "warp 9")):
-    print(f"-- {wname}: mean cycles between consecutive points, per iteration (us at 1965 MHz in brackets)")
+    print(f"-- {wname}: mean cycles between consecutive points, per iteration (us at the maximum SM clock, {clk:.0f} MHz, in brackets)")
     for b in range(IT):
         segs = []
         for k in range(1, 10):
