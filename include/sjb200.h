@@ -87,7 +87,9 @@ SJB200_API const char *sjb200_last_cuda_error(const sjb200_ctx *ctx);
  * "ew_min_bytes" (stage-1 launches of at least this size use the emit-warp build of the kernel; 0 = never),
  * "time_kernel" (0/1: record CUDA events around the scan kernel on its launch stream); none changes results */
 SJB200_API int sjb200_set_option(sjb200_ctx *ctx, const char *key, long value);
-/* "kernel_ms" (last scan kernel, needs time_kernel=1), "launches" (kernels launched by this context so far),
+/* "kernel_ms" (last scan kernel, needs time_kernel=1), "kernel_ms_mean" (the scan kernels since the previous query),
+ * both per document: a launch that scans several documents (sjb200_stage1_dev_batch) counts its duration divided by
+ * their number; "launches" (kernels launched by this context so far),
  * "ew_launches" (of which on the emit-warp build),
  * "grid_index", "sm_count"; negative when unavailable */
 SJB200_API double sjb200_get_stat(sjb200_ctx *ctx, const char *key);
@@ -121,8 +123,11 @@ SJB200_API int sjb200_stage1_dev(sjb200_ctx *ctx, const uint8_t *d_buf, size_t l
 SJB200_API int sjb200_minify_dev(sjb200_ctx *ctx, const uint8_t *d_buf, size_t len, uint8_t *d_dst, size_t *dst_len, void *stream);
 SJB200_API int sjb200_validate_utf8_dev(sjb200_ctx *ctx, const uint8_t *d_buf, size_t len, void *stream);
 
-/* many documents per call: all scans are queued back to back, one host wait, then each document's finish().
- * (what a caller with a corpus / NDJSON rows resident in HBM uses instead of a loop of sjb200_stage1_dev) */
+/* many documents per call: consecutive documents share one scan launch (up to 64 per launch), the launches are queued
+ * back to back, one host wait, then each document's finish().  A launch ends before a document whose input or index
+ * buffer overlaps the index buffer of an earlier document of the launch, or whose index buffer overlaps such a
+ * document's input, so results are those of a loop of sjb200_stage1_dev in order.
+ * (what a caller with a corpus / NDJSON rows resident in HBM uses instead of that loop) */
 typedef struct {
   const uint8_t *d_buf;          /* in: device pointer */
   size_t len;                    /* in */

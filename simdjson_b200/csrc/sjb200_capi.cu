@@ -59,7 +59,7 @@ struct sjb200_ctx {
   uint32_t *d_idx = nullptr;  size_t d_idx_words = 0;
   uint8_t *d_out = nullptr;   size_t d_out_bytes = 0;
   Carry *d_carry = nullptr;   // [kCarrySlots] one per chunk boundary of the chunked host pipeline
-  uint32_t *d_flags = nullptr;
+  uint32_t *d_flags = nullptr;  // [0] the launch's flags, [1 + slot] the flags of the document whose result goes to carry slot `slot`
   uint32_t *d_ticket = nullptr;
   unsigned long long *d_count_desc = nullptr;
   size_t desc_tiles = 0;
@@ -81,7 +81,12 @@ struct sjb200_ctx {
   cudaEvent_t ev_k0 = nullptr, ev_k1 = nullptr;  // around the last scan kernel when opt_time_kernel is set
   bool ev_valid = false;
   std::vector<cudaEvent_t> ev_pool;              // [2i], [2i+1] around launch i since the last kernel_ms_mean query
+  std::vector<uint32_t> ev_docs;                 // [i] documents launch i scanned
   size_t ev_used = 0;
+  uint32_t ev_last_docs = 1;                     // ... the launch around ev_k0 / ev_k1
+  // multi-document stage-1 launches: per group a DocEntry table and the documents' tensor maps, encoded for a whole
+  // batch round into pinned memory, copied group by group ahead of the launches
+  uint8_t *h_doctab = nullptr; uint8_t *d_doctab = nullptr; size_t doctab_bytes = 0;
   long opt_debug_timeline = 0;
   unsigned long long *d_debug = nullptr; size_t debug_tiles = 0; uint32_t debug_last_tiles = 0;
   unsigned long long launches = 0;               // kernels of ours launched by this context
@@ -149,9 +154,10 @@ void free_sized(sjb200_ctx *c) {
   c->desc_tiles = 0;
 }
 
-// look-back descriptors: sized for the capacity, zeroed once (epoch tags make them reusable)
-bool ensure_desc(sjb200_ctx *c, size_t len) {
-  const size_t need = std::max<size_t>(tiles_of(len), 1);
+// look-back descriptors: sized for the capacity, zeroed once (epoch tags make them reusable).  `need` descriptors: one per
+// tile is more than one per element.
+bool ensure_desc_n(sjb200_ctx *c, size_t need) {
+  need = std::max<size_t>(need, 1);
   if (need <= c->desc_tiles) return true;
   cudaFree(c->d_count_desc); c->d_count_desc = nullptr;
   c->desc_tiles = 0;
@@ -163,6 +169,7 @@ bool ensure_desc(sjb200_ctx *c, size_t len) {
   c->epoch = 0;
   return true;
 }
+bool ensure_desc(sjb200_ctx *c, size_t len) { return ensure_desc_n(c, tiles_of(len)); }
 
 // The wipe at the wrap of the 18-bit tag is ordered on the LAUNCH stream (a context is used on one stream at a time,
 // see sjb200.h): kernels queued earlier on it finish before the wipe, the next launch starts after it.
@@ -220,6 +227,29 @@ struct XchgTarget {
   uint32_t nranks, rank, slot, seq;
 };
 
+// Option time_kernel: events around one scan launch.  time_begin records the first one and returns the second (null:
+// not timed); time_end records the second.  `docs` = documents the launch scanned: kernel_ms / kernel_ms_mean report
+// its duration per document.
+cudaEvent_t time_begin(sjb200_ctx *c, cudaStream_t stream) {
+  if (!c->opt_time_kernel) return nullptr;
+  if (c->ev_used + 2 > c->ev_pool.size() && c->ev_pool.size() < 4096) {
+    cudaEvent_t a, b;
+    cudaEventCreate(&a); cudaEventCreate(&b);
+    c->ev_pool.push_back(a); c->ev_pool.push_back(b);
+    c->ev_docs.push_back(1);
+  }
+  if (c->ev_used + 2 > c->ev_pool.size()) return nullptr;
+  cudaEventRecord(c->ev_pool[c->ev_used], stream);
+  c->ev_used += 2;
+  return c->ev_pool[c->ev_used - 1];
+}
+void time_end(sjb200_ctx *c, cudaStream_t stream, cudaEvent_t e1, bool launched, uint32_t docs) {
+  if (!e1) return;
+  cudaEventRecord(e1, stream);
+  c->ev_docs[c->ev_used / 2 - 1] = docs;
+  c->ev_k0 = c->ev_pool[c->ev_used - 2]; c->ev_k1 = e1; c->ev_valid = launched; c->ev_last_docs = docs;
+}
+
 // Enqueue the scan of document tiles [tile_begin, tile_begin+ntiles) of (d_buf,len).
 bool enqueue_scan(sjb200_ctx *c, int kind, const CUtensorMap *map, bool tma, const uint8_t *d_buf, size_t len, uint32_t tile_begin,
                   uint32_t ntiles, bool has_last_tile, uint32_t prev_word, uint32_t *d_idx, uint8_t *d_dst, int carry_in_slot,
@@ -260,16 +290,7 @@ bool enqueue_scan(sjb200_ctx *c, int kind, const CUtensorMap *map, bool tma, con
     }
     if (c->d_debug) { cudaMemsetAsync(c->d_debug, 0, size_t(rows) * 64, stream); p.debug = c->d_debug; c->debug_last_tiles = rows; }
   }
-  cudaEvent_t e0 = nullptr, e1 = nullptr;
-  if (c->opt_time_kernel) {
-    if (c->ev_used + 2 > c->ev_pool.size() && c->ev_pool.size() < 4096) {
-      cudaEvent_t a, b;
-      cudaEventCreate(&a); cudaEventCreate(&b);
-      c->ev_pool.push_back(a); c->ev_pool.push_back(b);
-    }
-    if (c->ev_used + 2 <= c->ev_pool.size()) { e0 = c->ev_pool[c->ev_used]; e1 = c->ev_pool[c->ev_used + 1]; c->ev_used += 2; }
-    if (e0) cudaEventRecord(e0, stream);
-  }
+  cudaEvent_t e1 = time_begin(c, stream);
   bool launched;
   if (use_scan4(c, kind)) {
     const uint32_t tpe = uint32_t(scan4_tiles_per_element());
@@ -296,7 +317,7 @@ bool enqueue_scan(sjb200_ctx *c, int kind, const CUtensorMap *map, bool tma, con
     p.carry_out_host = host_out;
     launched = ok(c, launch_utf8v2(map, p, grid, stream), "launch utf8v2");
   }
-  if (e1) { cudaEventRecord(e1, stream); c->ev_k0 = e0; c->ev_k1 = e1; c->ev_valid = launched; }
+  time_end(c, stream, e1, launched, 1);
   c->launches += launched ? 1 : 0;
   return launched;
 }
@@ -346,10 +367,10 @@ extern "C" int sjb200_create(int device, size_t capacity, sjb200_ctx **out) {
   bool good = ok(c, cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking), "stream") &&
               ok(c, cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking), "stream") &&
               ok(c, cudaStreamCreateWithFlags(&c->out_stream, cudaStreamNonBlocking), "stream") &&
-              dev_alloc(c, &c->d_carry, kCarrySlots, "cudaMalloc(carry)") && dev_alloc(c, &c->d_flags, 1, "cudaMalloc(flags)") &&
+              dev_alloc(c, &c->d_carry, kCarrySlots, "cudaMalloc(carry)") && dev_alloc(c, &c->d_flags, 1 + kCarrySlots, "cudaMalloc(flags)") &&
               dev_alloc(c, &c->d_ticket, 4, "cudaMalloc(ticket)") &&
               ok(c, cudaMemset(c->d_ticket, 0, 4 * sizeof(uint32_t)), "memset ticket") &&
-              ok(c, cudaMemset(c->d_flags, 0, sizeof(uint32_t)), "memset flags");
+              ok(c, cudaMemset(c->d_flags, 0, (1 + kCarrySlots) * sizeof(uint32_t)), "memset flags");
   void *hp = nullptr;
   good = good && ok(c, cudaMallocHost(&hp, kCarrySlots * sizeof(Carry)), "cudaMallocHost");
   c->h_carry = static_cast<Carry *>(hp);
@@ -393,7 +414,8 @@ extern "C" void sjb200_destroy(sjb200_ctx *c) {
   DeviceGuard g(c->device);
   if (c->stream) cudaStreamSynchronize(c->stream);
   free_sized(c);
-  cudaFree(c->d_carry); cudaFree(c->d_flags); cudaFree(c->d_ticket); cudaFree(c->d_sfin); cudaFree(c->d_doc_scratch); cudaFree(c->d_ndocs); cudaFree(c->d_tok_scratch); cudaFree(c->d_tok_tot); cudaFree(c->d_tails); cudaFree(c->d_tail_ptrs); cudaFree(c->d_debug); cudaFree(c->d_park);
+  cudaFree(c->d_carry); cudaFree(c->d_flags); cudaFree(c->d_ticket); cudaFree(c->d_sfin); cudaFree(c->d_doc_scratch); cudaFree(c->d_ndocs); cudaFree(c->d_tok_scratch); cudaFree(c->d_tok_tot); cudaFree(c->d_tails); cudaFree(c->d_tail_ptrs); cudaFree(c->d_debug); cudaFree(c->d_park); cudaFree(c->d_doctab);
+  if (c->h_doctab) cudaFreeHost(c->h_doctab);
   if (c->h_carry) cudaFreeHost(c->h_carry);
   if (c->h_flags) cudaFreeHost(c->h_flags);
   if (c->h_small) cudaFreeHost(c->h_small);
@@ -450,20 +472,20 @@ extern "C" int sjb200_unpin_host_memory(sjb200_ctx *c, void *ptr) {
 
 extern "C" double sjb200_get_stat(sjb200_ctx *c, const char *key) {
   if (!c || !key) return -1.0;
-  if (!strcmp(key, "kernel_ms")) {  // duration of the last scan kernel (needs option time_kernel=1 and a finished call)
+  if (!strcmp(key, "kernel_ms")) {  // duration of the last scan kernel per document it scanned (needs option time_kernel=1 and a finished call)
     if (!c->ev_valid) return -1.0;
     DeviceGuard g(c->device);
     float ms = 0.f;
     if (cudaEventElapsedTime(&ms, c->ev_k0, c->ev_k1) != cudaSuccess) { (void)cudaGetLastError(); return -1.0; }
-    return double(ms);
+    return double(ms) / double(c->ev_last_docs);
   }
-  if (!strcmp(key, "kernel_ms_mean")) {  // mean duration of the scan kernels launched since the previous query
+  if (!strcmp(key, "kernel_ms_mean")) {  // scan kernel time per document, over the kernels launched since the previous query
     DeviceGuard g(c->device);
     double sum = 0;
     size_t n = 0;
     for (size_t i = 0; i + 1 < c->ev_used; i += 2) {
       float ms = 0.f;
-      if (cudaEventElapsedTime(&ms, c->ev_pool[i], c->ev_pool[i + 1]) == cudaSuccess) { sum += ms; n++; } else (void)cudaGetLastError();
+      if (cudaEventElapsedTime(&ms, c->ev_pool[i], c->ev_pool[i + 1]) == cudaSuccess) { sum += ms; n += c->ev_docs[i / 2]; } else (void)cudaGetLastError();
     }
     c->ev_used = 0;
     c->ev_valid = false;
@@ -508,26 +530,45 @@ extern "C" int sjb200_set_option(sjb200_ctx *c, const char *key, long value) {
 
 // =============================================================================== device-resident
 namespace {
-// enqueue one device-resident stage-1 scan; its {count,state,flags} come back in h_carry[slot]
-void stage1_enqueue_into(sjb200_ctx *c, PendingCall &pc, const uint8_t *d_buf, size_t len, int mode, uint32_t *d_idx, cudaStream_t s,
-                         int slot, const uint8_t *tail3 = nullptr /* host copy of the last min(3, len) bytes, when the caller fetched it */) {
+// The checks before a device-resident stage-1 scan and the trim of a partial UTF-8 tail (json_structural_indexer.h
+// L195-204).  False: the call ends here, with pc.early_error.
+bool stage1_prepare(sjb200_ctx *c, PendingCall &pc, const uint8_t *d_buf, size_t len, int mode, uint32_t *d_idx, cudaStream_t s, int slot,
+                    const uint8_t *tail3 /* host copy of the last min(3, len) bytes, when the caller fetched it */) {
   pc = PendingCall();
   pc.kind = kIndex; pc.mode = mode; pc.d_buf = d_buf; pc.d_idx = d_idx; pc.stream = s; pc.len = len; pc.carry_slot = slot;
-  if (mode < SJB200_REGULAR || mode > SJB200_COMMA_DELIMITED_FINAL) { pc.early_error = SJB200_UNEXPECTED_ERROR; return; }
-  if (len > c->capacity) { pc.early_error = SJB200_CAPACITY; return; }   // json_structural_indexer.h L195
-  if (len == 0) { pc.early_error = SJB200_EMPTY; return; }                // L197
-  if (mode != SJB200_REGULAR) {                                           // L198-204
+  if (mode < SJB200_REGULAR || mode > SJB200_COMMA_DELIMITED_FINAL) { pc.early_error = SJB200_UNEXPECTED_ERROR; return false; }
+  if (len > c->capacity) { pc.early_error = SJB200_CAPACITY; return false; }   // json_structural_indexer.h L195
+  if (len == 0) { pc.early_error = SJB200_EMPTY; return false; }                // L197
+  if (mode != SJB200_REGULAR) {                                                 // L198-204
     const size_t k = std::min<size_t>(3, len);
     if (!tail3) {
       if (!ok(c, cudaMemcpyAsync(c->h_small, d_buf + len - k, k, cudaMemcpyDeviceToHost, s), "D2H tail") ||
           !ok(c, cudaStreamSynchronize(s), "sync"))
-        { pc.early_error = SJB200_UNEXPECTED_ERROR; return; }
+        { pc.early_error = SJB200_UNEXPECTED_ERROR; return false; }
       tail3 = c->h_small;
     }
     len = trim_partial_utf8_tail(tail3, k, len);
     pc.len = len;
-    if (len == 0) { pc.early_error = SJB200_UTF8_ERROR; return; }
+    if (len == 0) { pc.early_error = SJB200_UTF8_ERROR; return false; }
   }
+  return true;
+}
+
+// whitespace-separated streams: the rest of finish() (find_next_document_index, the final fix-up) runs on the device
+// right behind the scan -- no host round trip between the two (sjb200_docs.cu)
+void stage1_stream_epilogue(sjb200_ctx *c, PendingCall &pc) {
+  if (pc.mode == SJB200_STREAMING_PARTIAL || pc.mode == SJB200_STREAMING_FINAL) {
+    c->launches++;
+    const int slot = pc.carry_slot;
+    if (!ok(c, launch_stream_finish(pc.d_buf, pc.d_idx, c->d_carry + slot, uint32_t(pc.len), pc.mode, c->d_sfin + slot, c->h_sfin + slot, pc.stream), "stream finish"))
+      pc.early_error = SJB200_UNEXPECTED_ERROR;
+  }
+}
+
+// enqueue one device-resident stage-1 scan; its {count,state,flags} come back in h_carry[slot]
+void stage1_enqueue_into(sjb200_ctx *c, PendingCall &pc, const uint8_t *d_buf, size_t len, int mode, uint32_t *d_idx, cudaStream_t s, int slot) {
+  if (!stage1_prepare(c, pc, d_buf, len, mode, d_idx, s, slot, nullptr)) return;
+  len = pc.len;
   if (!ensure_desc(c, len)) { pc.early_error = SJB200_MEMALLOC; return; }
   CUtensorMap map;
   bool tma = false;
@@ -538,13 +579,7 @@ void stage1_enqueue_into(sjb200_ctx *c, PendingCall &pc, const uint8_t *d_buf, s
       (!use_scan4(c, kIndex) &&
        !ok(c, cudaMemcpyAsync(c->h_carry + slot, c->d_carry + slot, sizeof(Carry), cudaMemcpyDeviceToHost, s), "D2H result")))
     { pc.early_error = SJB200_UNEXPECTED_ERROR; return; }
-  // whitespace-separated streams: the rest of finish() (find_next_document_index, the final fix-up) runs on the device
-  // right behind the scan -- no host round trip between the two (sjb200_docs.cu)
-  if (mode == SJB200_STREAMING_PARTIAL || mode == SJB200_STREAMING_FINAL) {
-    c->launches++;
-    if (!ok(c, launch_stream_finish(d_buf, d_idx, c->d_carry + slot, uint32_t(len), mode, c->d_sfin + slot, c->h_sfin + slot, s), "stream finish"))
-      pc.early_error = SJB200_UNEXPECTED_ERROR;
-  }
+  stage1_stream_epilogue(c, pc);
 }
 
 // complete one enqueued scan (the stream has been synchronised by the caller)
@@ -619,8 +654,128 @@ extern "C" int sjb200_stage1_dev_finish(sjb200_ctx *c, uint32_t *n_inout) {
   return stage1_finish_from(c, pc, n_inout);
 }
 
-// Many documents in one call (NDJSON rows, a corpus): every scan is queued back to back on the stream, the host
-// waits once, then completes each document's finish() logic.  docs[i].error receives the error_code.
+namespace {
+bool ranges_overlap(const void *a, size_t an, const void *b, size_t bn) {
+  const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
+  return x < y + bn && y < x + an;
+}
+size_t out_bytes(const PendingCall &pc) { return 4 * (pc.len + 3); }  // at most len structurals + 3 sentinels
+
+// Enqueue the scans of the prepared calls (those without an early error), consecutive documents grouped into one
+// multi-document launch each.  A group ends before a document that reads or writes memory an earlier document of the
+// group writes, or writes memory it reads: the launches then keep the order of a one-by-one loop.  The tables of all
+// groups are encoded into pinned memory first; each is copied ahead of its launch, nothing waits for the device.
+int enqueue_doc_groups(sjb200_ctx *c, std::vector<PendingCall> &calls, cudaStream_t s) {
+  constexpr uint64_t kMaxGroupElems = 1u << 20;  // 64 GiB of input; 8 MiB of look-back descriptors
+  const uint32_t tpe = uint32_t(scan4_tiles_per_element());
+  auto elems_of = [&](const PendingCall &pc) { return uint64_t((tiles_of(pc.len) + tpe - 1) / tpe); };
+  std::vector<std::vector<int>> groups;
+  uint64_t g_elems = 0, max_elems = 0;
+  for (int i = 0; i < int(calls.size()); i++) {
+    const PendingCall &pc = calls[size_t(i)];
+    if (pc.early_error >= 0) continue;
+    bool split = groups.empty() || groups.back().size() == size_t(kMaxLaunchDocs) || g_elems + elems_of(pc) > kMaxGroupElems;
+    for (size_t k = 0; !split && k < groups.back().size(); k++) {
+      const PendingCall &q = calls[size_t(groups.back()[k])];
+      split = ranges_overlap(pc.d_buf, pc.len, q.d_idx, out_bytes(q)) || ranges_overlap(pc.d_idx, out_bytes(pc), q.d_idx, out_bytes(q)) ||
+              ranges_overlap(pc.d_idx, out_bytes(pc), q.d_buf, q.len);
+    }
+    if (split) { groups.emplace_back(); g_elems = 0; }
+    groups.back().push_back(i);
+    g_elems += elems_of(pc);
+    max_elems = std::max(max_elems, g_elems);
+  }
+  if (groups.empty()) return SJB200_SUCCESS;
+  if (!ensure_desc_n(c, max_elems)) return SJB200_MEMALLOC;
+  // table layout of group g at offset off[g]: ndocs DocEntry, then ndocs tensor maps (64-byte aligned)
+  std::vector<size_t> off(groups.size() + 1, 0);
+  for (size_t g = 0; g < groups.size(); g++) {
+    const size_t n = groups[g].size() > 1 ? groups[g].size() : 0;  // a group of one is an ordinary single-document launch
+    off[g + 1] = off[g] + ((n * sizeof(DocEntry) + 127) & ~size_t(127)) + n * sizeof(CUtensorMap);
+  }
+  if (off.back() > c->doctab_bytes) {
+    if (c->h_doctab) cudaFreeHost(c->h_doctab);
+    cudaFree(c->d_doctab);
+    c->h_doctab = nullptr; c->d_doctab = nullptr; c->doctab_bytes = 0;
+    void *hp = nullptr;
+    if (!ok(c, cudaMallocHost(&hp, off.back()), "cudaMallocHost(doc tables)") || !dev_alloc(c, &c->d_doctab, off.back(), "cudaMalloc(doc tables)"))
+      return SJB200_MEMALLOC;
+    c->h_doctab = static_cast<uint8_t *>(hp);
+    c->doctab_bytes = off.back();
+  }
+  static_assert(sizeof(DocEntry) == 64 && sizeof(CUtensorMap) == 128, "table layout");
+  for (size_t g = 0; g < groups.size(); g++) {
+    const std::vector<int> &G = groups[g];
+    if (G.size() == 1) {
+      PendingCall &pc = calls[size_t(G[0])];
+      CUtensorMap map;
+      bool tma = false;
+      map_for(c, kIndex, &map, pc.d_buf, pc.len, &tma);
+      if (!enqueue_scan(c, kIndex, &map, tma, pc.d_buf, pc.len, 0, tiles_of(pc.len), true, 0x20202020u, pc.d_idx, nullptr, -1, s, pc.carry_slot, true,
+                        nullptr, c->h_carry + pc.carry_slot))
+        pc.early_error = SJB200_UNEXPECTED_ERROR;
+      else
+        stage1_stream_epilogue(c, pc);
+      continue;
+    }
+    const size_t n = G.size();
+    DocEntry *he = reinterpret_cast<DocEntry *>(c->h_doctab + off[g]);
+    const size_t maps_at = off[g] + ((n * sizeof(DocEntry) + 127) & ~size_t(127));
+    CUtensorMap *hm = reinterpret_cast<CUtensorMap *>(c->h_doctab + maps_at);
+    const CUtensorMap *dm = reinterpret_cast<const CUtensorMap *>(c->d_doctab + maps_at);
+    uint32_t elems = 0, tiles = 0;
+    for (size_t k = 0; k < n; k++) {
+      const PendingCall &pc = calls[size_t(G[k])];
+      bool tma = false;
+      map_for(c, kIndex, &hm[k], pc.d_buf, pc.len, &tma);
+      DocEntry &e = he[k];
+      e.buf = pc.d_buf;
+      e.idx_out = pc.d_idx;
+      e.carry_out = c->d_carry + pc.carry_slot;
+      e.carry_out_host = c->h_carry + pc.carry_slot;
+      e.flags = c->d_flags + 1 + pc.carry_slot;
+      e.tmap = tma ? static_cast<const void *>(dm + k) : nullptr;
+      e.len = uint32_t(pc.len);
+      e.scan_end = uint32_t(pc.len);
+      e.first_elem = elems;
+      e.nelem = uint32_t(elems_of(pc));
+      elems += e.nelem;
+      tiles += tiles_of(pc.len);
+    }
+    ScanParams p;
+    memset(&p, 0, sizeof(p));
+    p.prev_word = 0x20202020u;
+    p.check_eof = 1;
+    p.write_sentinels = 1;
+    p.ntiles = tiles;
+    p.flags = c->d_flags;
+    p.count_desc = c->d_count_desc;
+    p.ticket = c->d_ticket;
+    p.docs = reinterpret_cast<const DocEntry *>(c->d_doctab + off[g]);
+    p.ndocs = uint32_t(n);
+    bool good = next_epoch(c, s, &p.epoch) &&
+                ok(c, cudaMemcpyAsync(c->d_doctab + off[g], c->h_doctab + off[g], off[g + 1] - off[g], cudaMemcpyHostToDevice, s), "H2D doc table");
+    if (good) {
+      CUtensorMap unused;
+      memset(&unused, 0, sizeof(unused));
+      cudaEvent_t e1 = time_begin(c, s);
+      good = ok(c, launch_scan4(&unused, p, grid_for(c, kIndex, elems), 0, s), "launch scan4 (documents)");
+      time_end(c, s, e1, good, uint32_t(n));
+      c->launches += good ? 1 : 0;
+    }
+    for (size_t k = 0; k < n; k++) {
+      PendingCall &pc = calls[size_t(G[k])];
+      if (good) stage1_stream_epilogue(c, pc);
+      else pc.early_error = SJB200_UNEXPECTED_ERROR;
+    }
+  }
+  return SJB200_SUCCESS;
+}
+}  // namespace
+
+// Many documents in one call (NDJSON rows, a corpus): consecutive documents share a scan launch where their memory
+// allows it (enqueue_doc_groups), the launches are queued back to back on the stream, the host waits once, then
+// completes each document's finish() logic.  docs[i].error receives the error_code.
 extern "C" int sjb200_stage1_dev_batch(sjb200_ctx *c, sjb200_doc *docs, int ndocs, int mode, void *stream) {
   if (!c || (!docs && ndocs > 0) || ndocs < 0) return SJB200_UNEXPECTED_ERROR;
   DeviceGuard g(c->device);
@@ -660,8 +815,10 @@ extern "C" int sjb200_stage1_dev_batch(sjb200_ctx *c, sjb200_doc *docs, int ndoc
     }
     for (int i = 0; i < group; i++) {
       sjb200_doc &d = docs[done + i];
-      stage1_enqueue_into(c, calls[size_t(i)], d.d_buf, d.len, mode, d.d_idx, s, 1 + i, tails ? tails + 4 * size_t(i) : nullptr);
+      stage1_prepare(c, calls[size_t(i)], d.d_buf, d.len, mode, d.d_idx, s, 1 + i, tails ? tails + 4 * size_t(i) : nullptr);
     }
+    const int rc = enqueue_doc_groups(c, calls, s);
+    if (rc != SJB200_SUCCESS) return rc;
     if (!ok(c, cudaStreamSynchronize(s), "sync")) return SJB200_UNEXPECTED_ERROR;
     for (int i = 0; i < group; i++) {
       sjb200_doc &d = docs[done + i];

@@ -30,6 +30,23 @@ struct Carry {
   uint32_t reserved;
 };
 
+// One document of a multi-document stage-1 launch (ScanParams::docs).  Its elements are the launch's elements
+// [first_elem, first_elem + nelem): tickets and look-back descriptors run over the concatenation of the documents.
+// A single-document launch builds the one entry from the scalar fields of ScanParams.
+struct DocEntry {
+  const uint8_t *buf;
+  uint32_t *idx_out;
+  Carry *carry_out;
+  Carry *carry_out_host;    // optional pinned host mirror of carry_out
+  uint32_t *flags;          // kFlag* bits of this document (zero between launches; the last CTA moves them to carry_out)
+  const void *tmap;         // null: plain loads.  Else the document's tensor map (4 KiB boxes), 64-byte aligned in global memory
+  uint32_t len;             // document length in bytes (>= 1)
+  uint32_t scan_end;        // min(len, end of the launch's tile range): blocks at or beyond it are not this launch's
+  uint32_t first_elem;
+  uint32_t nelem;
+};
+constexpr int kMaxLaunchDocs = 64;  // documents per multi-document launch (their table is copied into every CTA's shared memory)
+
 struct ScanParams {
   const uint8_t *buf;       // device pointer to byte 0 of the document (or shard)
   uint64_t len;             // document length in bytes (<= 4 GiB - 1); bytes past it read as 0x20
@@ -56,6 +73,12 @@ struct ScanParams {
   // the path's one exchange step (SURVEY.md 8e) without a collective launch.  xchg_nranks == 0: no exchange.
   unsigned long long *xchg_peer[kMaxRanks];  // [r] = base of rank r's window: [slots][kMaxRanks][2] words
   uint32_t xchg_nranks, xchg_rank, xchg_slot, xchg_seq;
+  // scan4 stage 1, several whole documents in one launch: ndocs (1..kMaxLaunchDocs) entries in device memory.  buf, len,
+  // use_tma, idx_out, carry_out and carry_out_host are then unused; tile_begin = 0, no carry-in, no exchange, pos_base = 0,
+  // prev_word = 0x20202020, check_eof = write_sentinels = 1, and `flags` only collects what concerns the whole launch.
+  // ndocs = 0: one document described by the scalar fields above.
+  const DocEntry *docs;
+  uint32_t ndocs;
 };
 
 #if defined(__CUDACC__)

@@ -27,6 +27,9 @@
 //     load of its next block is always in flight.  A second schedule ("deferred": masks parked in an L2-resident
 //     scratch ring, all emits after the CTA's last scan) is kept as an option.
 //   * All arithmetic is the bit-plane algebra of sjb200_bits.cuh: 32 bytes per LOP3, no per-byte code.
+//   * Stage 1 may scan several whole documents in one launch (ScanParams::docs): tickets and descriptors run over the
+//     concatenation of their elements, every slot carries its element's document (Smem::tdoc), and each document is
+//     finalised by the chain warp that resolves its last element.  A single-document launch is the one-entry case.
 //
 // The same source compiles for the host SIMT emulation (SJB200_HOST_EMU, tests/simt_emul.cpp), which runs it with one
 // OS thread per CUDA thread against the oracle on machines without a GPU.
@@ -103,7 +106,10 @@ struct Smem {
   sj_u4 park[kGPark > 0 ? 1 : kPark][2][kGPark > 0 ? 1 : kScanWarps * 32];  // [pipeline buffer][polarity][thread]: candidate structural masks (shared-memory parking)
   uint32_t parkpre[kGPark > 0 ? 1 : kPark][kGPark > 0 ? 1 : kScanWarps * 32];  // exclusive prefix of the lane's counts inside its block, both polarities packed
   uint32_t compact_lut[16];                   // minify: see compact_entry
+  alignas(16) DocEntry doc[kMaxLaunchDocs];   // the launch's documents (a single-document launch: entry 0 from ScanParams)
+  uint32_t ndocs;
   uint32_t ticket[kNS];
+  uint32_t tdoc[kNS];                         // document of the element in the slot
   uint32_t summary[kNS][kScanWarps];          // c0 | c1<<16 | parity<<29 | ctl-hit0<<30 | ctl-hit1<<31
   uint32_t arrived[kNS];                      // scan warps done with the element (the last one composes and publishes)
   uint32_t elem[kNS][4];                      // composed element: quote parity, outputs entered outside / inside a string, ctl hits (bit0/1)
@@ -253,7 +259,7 @@ SJ_DEV uint64_t run_forward(const uint8_t *buf, uint64_t begin, uint64_t limit, 
 // pos-1), bit2 = byte pos-1 is a "non-quote scalar" (json_scanner.h L148-149).  Exact for any input: the run is
 // followed back as far as it goes, at most to the first byte of this launch, where the launch's carry-in takes over.
 // `b1` = byte pos-1.  Warp-uniform.
-SJ_DEV uint32_t boundary_state(const ScanParams &p, uint64_t pos, uint64_t launch_start, uint32_t cin_state, uint32_t pw, unsigned lane) {
+SJ_DEV uint32_t boundary_state(const uint8_t *buf, uint64_t pos, uint64_t launch_start, uint32_t cin_state, uint32_t pw, unsigned lane) {
   if (pos == launch_start) return cin_state & 5u;
   const uint32_t b1 = pw >> 24;
   if (b1 != 0x5Cu && b1 != 0x22u) return byte_is_scalar(b1) ? 4u : 0u;  // the common case: one byte decides
@@ -279,7 +285,7 @@ SJ_DEV uint32_t boundary_state(const ScanParams &p, uint64_t pos, uint64_t launc
   } else {
     const uint64_t end = isq ? pos - 1 : pos;
     bool hit = false;
-    const uint64_t r = run_back(p.buf, end, launch_start, lane, &hit);
+    const uint64_t r = run_back(buf, end, launch_start, lane, &hit);
     odd = uint32_t(r + ((hit && (cin_state & 1u)) ? 1u : 0u)) & 1u;
   }
   if (isq) return odd << 2;  // escaped quote = scalar byte; a real quote is not; neither escapes what follows
@@ -287,12 +293,12 @@ SJ_DEV uint32_t boundary_state(const ScanParams &p, uint64_t pos, uint64_t launc
 }
 
 // the 4 bytes before document offset `pos` as a little-endian word (byte pos-1 on top)
-SJ_DEV uint32_t word_before(const ScanParams &p, uint64_t pos) {
-  if (pos == 0) return p.prev_word;
-  if (pos >= 4 && ((reinterpret_cast<uintptr_t>(p.buf) + pos) & 3u) == 0) return sj_ldg_u32(p.buf + pos - 4);
+SJ_DEV uint32_t word_before(const uint8_t *buf, uint32_t prev_word, uint64_t pos) {
+  if (pos == 0) return prev_word;
+  if (pos >= 4 && ((reinterpret_cast<uintptr_t>(buf) + pos) & 3u) == 0) return sj_ldg_u32(buf + pos - 4);
   uint32_t w = 0;
   for (int d = 1; d <= 4; d++) {
-    const uint32_t b = (pos >= uint64_t(d)) ? sj_ldg_u8(p.buf + pos - d) : ((p.prev_word >> (8 * (4 - d + int(pos)))) & 0xFFu);
+    const uint32_t b = (pos >= uint64_t(d)) ? sj_ldg_u8(buf + pos - d) : ((prev_word >> (8 * (4 - d + int(pos)))) & 0xFFu);
     w |= b << (8 * (4 - d));
   }
   return w;
@@ -301,20 +307,20 @@ SJ_DEV uint32_t word_before(const ScanParams &p, uint64_t pos) {
 // ------------------------------------------------------------------------------------------------ block I/O
 // A warp copies one block global -> shared in the swizzled layout, padding with 0x20 past len.  Used for the last
 // (partial) block and for buffers TMA cannot address (stage 1 never reads past len: buf_block_reader.h L98-104).
-SJ_DEV void fill_block_guarded(uint8_t *T, const ScanParams &p, uint64_t bstart, unsigned lane) {
-  const bool aligned = (reinterpret_cast<uintptr_t>(p.buf) & 15u) == 0;
+SJ_DEV void fill_block_guarded(uint8_t *T, const uint8_t *buf, uint64_t len, uint64_t bstart, unsigned lane) {
+  const bool aligned = (reinterpret_cast<uintptr_t>(buf) & 15u) == 0;
   for (uint32_t c = lane; c < uint32_t(kBlockBytes / 16); c += 32) {
     const uint64_t g = bstart + uint64_t(c) * 16;
     sj_u4 v;
-    if (aligned && g + 16 <= p.len) {
-      v = sj_ldg_u4(p.buf + g);
+    if (aligned && g + 16 <= len) {
+      v = sj_ldg_u4(buf + g);
     } else {
       uint32_t w[4];
       for (int k = 0; k < 4; k++) {
         uint32_t x = 0;
         for (int b = 0; b < 4; b++) {
           const uint64_t q = g + 4 * k + b;
-          const uint32_t byte = (q < p.len) ? sj_ldg_u8(p.buf + q) : 0x20u;
+          const uint32_t byte = (q < len) ? sj_ldg_u8(buf + q) : 0x20u;
           x |= byte << (8 * b);
         }
         w[k] = x;
@@ -339,7 +345,7 @@ SJ_DEV void load_unit(const uint8_t *T, uint32_t off, uint32_t w[8]) {
 // kMin: the minify flavour (json_minifier.h L68-97): no UTF-8 validation, the two candidate masks are the bytes to KEEP
 // (everything but whitespace outside strings) among the first `valid_bytes` of the block, the counts are bytes.
 template <bool kMin>
-SJ_DEV uint32_t scan_block(const uint8_t *T, uint32_t pw0, uint32_t e_in, uint32_t c_in, unsigned lane, const ScanParams &p, sj_u4 *park0,
+SJ_DEV uint32_t scan_block(const uint8_t *T, uint32_t pw0, uint32_t e_in, uint32_t c_in, unsigned lane, uint32_t *flags, sj_u4 *park0,
                            sj_u4 *park1, uint32_t *parkpre, uint32_t valid_bytes) {
   const uint32_t lane_off = lane * 128u;
   uint32_t bs[4], qu[4], op[4], sc[4], cl[4];
@@ -388,7 +394,7 @@ SJ_DEV uint32_t scan_block(const uint8_t *T, uint32_t pw0, uint32_t e_in, uint32
       }
     }
   }
-  if (!kMin && sj_any(uerr != 0) && lane == 0) sj_atomic_or(p.flags, kFlagUtf8);
+  if (!kMin && sj_any(uerr != 0) && lane == 0) sj_atomic_or(flags, kFlagUtf8);
 
   // ---- escapes: which quotes are real (json_escape_scanner.h L96-143, resolved across lanes with one addition)
   uint32_t qr[4];
@@ -525,9 +531,10 @@ SJ_DEV void emit_block(Smem *S, const ScanParams &p, uint64_t out_base, uint32_t
   const uint32_t total = pol ? ((sum >> 16) & 0x1FFFu) : (sum & 0xFFFFu);
   if (total == 0) return;
   const uint32_t elem = S->ticket[ns];
+  const DocEntry &D = S->doc[S->tdoc[ns]];
   const uint32_t off = (prew >> (16 * pol)) & 0xFFFFu;
-  const uint32_t pos_lane = p.pos_base + p.tile_begin * uint32_t(kTileBytes) + elem * uint32_t(kElemBytes) + warp * uint32_t(kBlockBytes) + lane * 128u;
-  uint32_t *out = p.idx_out + (out_base + S->res_base[ns][warp]);
+  const uint32_t pos_lane = p.pos_base + p.tile_begin * uint32_t(kTileBytes) + (elem - D.first_elem) * uint32_t(kElemBytes) + warp * uint32_t(kBlockBytes) + lane * 128u;
+  uint32_t *out = D.idx_out + (out_base + S->res_base[ns][warp]);
   if (total + 3 <= kStageWords) {
     // positions go to shared memory (scattered 4-byte global stores cost one L1 wavefront each) and leave as coalesced
     // 16-byte vectors: the staging area starts at the same offset modulo 4 words as the destination, so the aligned
@@ -608,7 +615,7 @@ SJ_DEV bool emit_minify_block(Smem *S, const sj_tensor_map *tmap, const ScanPara
     wait_bar(bar, parity, p, 32);
   } else {
     if (total == 0) return false;
-    fill_block_guarded(slot, p, bstart, lane);
+    fill_block_guarded(slot, p.buf, p.len, bstart, lane);  // (minify launches have one document)
     sj_syncwarp();
   }
   if (total == 0) return by_tma;
@@ -685,7 +692,7 @@ SJ_DEV bool emit_minify_block(Smem *S, const sj_tensor_map *tmap, const ScanPara
 // Run by the LAST scan warp to finish an element (so the aggregate is out as early as possible, independent of how far
 // the chain warp is with older elements): compose the block summaries for either polarity at the start of the
 // element, publish the aggregate in the look-back chain, leave the per-block prefixes for the chain warp.
-SJ_DEV void compose_element(Smem *S, const ScanParams &p, int ns, uint32_t t, unsigned lane) {
+SJ_DEV void compose_element(Smem *S, const ScanParams &p, int ns, uint32_t t, uint32_t doc_first, unsigned lane) {
   // Lane w holds the summary of block w.  Only one bit is order-dependent: the quote parities of the blocks are one
   // ballot word, the polarity entering block w (for an element entered outside a string) is a popcount, and what a block
   // contributes for either polarity of the element is then known per lane -- the element's aggregate is two REDUX sums.
@@ -700,7 +707,7 @@ SJ_DEV void compose_element(Smem *S, const ScanParams &p, int ns, uint32_t t, un
   const uint32_t HA = sj_any((s ? h1 : h0) != 0) ? 1u : 0u, HB = sj_any((s ? h0 : h1) != 0) ? 1u : 0u;
   const uint32_t par = uint32_t(sj_popc(P)) & 1u;
   if (lane == 0) {
-    if (t > 0) sj_st_relaxed_u64(p.count_desc + t, pack_agg(p.epoch, par, A, B));  // element 0 goes straight to inclusive
+    if (t > doc_first) sj_st_relaxed_u64(p.count_desc + t, pack_agg(p.epoch, par, A, B));  // a document's first element goes straight to inclusive
     S->elem[ns][0] = par;
     S->elem[ns][1] = A;
     S->elem[ns][2] = B;
@@ -720,9 +727,14 @@ SJ_DEV void compose_element(Smem *S, const ScanParams &p, int ns, uint32_t t, un
 }
 
 // ------------------------------------------------------------------------------------------------ scan warps
-SJ_DEV void publish_ticket(Smem *S, uint32_t j, uint32_t value, unsigned lane) {
+// Publishes ticket `value` in slot j with its document: the first one at or after `hint` (the document of the CTA's
+// previous ticket -- a CTA's tickets increase) whose successor starts beyond it.
+SJ_DEV void publish_ticket(Smem *S, uint32_t j, uint32_t value, uint32_t hint, unsigned lane) {
   if (lane == 0) {
+    uint32_t d = hint;
+    while (d + 1 < S->ndocs && S->doc[d + 1].first_elem <= value) d++;
     S->ticket[j % kNS] = value;
+    S->tdoc[j % kNS] = d;
     sj_mbar_arrive(&S->ticket_ready[j % kNS]);
   }
   sj_syncwarp();
@@ -733,21 +745,29 @@ SJ_DEV uint32_t wait_ticket(Smem *S, uint32_t j, const ScanParams &p) {
   return S->ticket[j % kNS];
 }
 
-// start the load of block `warp` of element `elem` into ring slot r; returns true when it arrives by TMA
-SJ_DEV bool issue_load(Smem *S, const sj_tensor_map *tmap, const ScanParams &p, uint32_t elem, unsigned warp, unsigned lane, int r,
-                       uint32_t *pw_out, uint64_t scan_limit) {
-  const uint64_t bstart = uint64_t(p.tile_begin) * kTileBytes + uint64_t(elem) * kElemBytes + uint64_t(warp) * kBlockBytes;
+// elements of the launch, over all its documents
+SJ_DEV uint32_t launch_elements(const Smem *S) { return S->doc[S->ndocs - 1].first_elem + S->doc[S->ndocs - 1].nelem; }
+
+// start the load of block `warp` of local element `le` of document d into ring slot r; returns true when it arrives by
+// TMA.  *fenced: the last document whose tensor map (written by the host into global memory) this thread has fenced.
+SJ_DEV bool issue_load(Smem *S, uint32_t d, const ScanParams &p, uint32_t le, unsigned warp, unsigned lane, int r, uint32_t *pw_out, uint32_t *fenced) {
+  const DocEntry &D = S->doc[d];
+  const uint64_t bstart = uint64_t(p.tile_begin) * kTileBytes + uint64_t(le) * kElemBytes + uint64_t(warp) * kBlockBytes;
   const uint64_t row = bstart / 128;
-  const bool full = p.use_tma && bstart < scan_limit && (row + kBlockRows <= p.len / 128);
+  const bool full = D.tmap != nullptr && bstart < D.scan_end && (row + kBlockRows <= D.len / 128);
   sj_syncwarp();  // every lane is done with the slot (previous block, emit staging)
   if (lane == 0) {
     if (full) {
+      if (p.ndocs > 0 && d != *fenced) {
+        sj_fence_tensormap_acquire(D.tmap);
+        *fenced = d;
+      }
       sj_fence_proxy_async();
       sj_mbar_arrive_expect_tx(&S->full[warp][r], kBlockBytes);
-      sj_tma_load_rows(S->ring[warp][r], tmap, &S->full[warp][r], uint32_t(row));
+      sj_tma_load_rows(S->ring[warp][r], static_cast<const sj_tensor_map *>(D.tmap), &S->full[warp][r], uint32_t(row));
     }
     // after the TMA is on its way: the fence above would otherwise sit out this load's round trip to L2
-    *pw_out = (bstart < p.len) ? word_before(p, bstart) : 0x20202020u;
+    *pw_out = (bstart < D.len) ? word_before(D.buf, p.prev_word, bstart) : 0x20202020u;
   }
   return full;
 }
@@ -759,10 +779,8 @@ SJ_DEV void emit_role(Smem *S, const sj_tensor_map *tmap, const ScanParams &p, c
 // kMode: 0 stage 1; 2 minify
 template <int kMode>
 SJ_DEV void scan_role(Smem *S, const sj_tensor_map *tmap, const ScanParams &p, const Carry &cin, unsigned warp, unsigned lane, uint32_t first_ticket) {
-  const uint32_t nelem = elements_of(p);
+  const uint32_t nelem = launch_elements(S);
   const uint64_t launch_start = uint64_t(p.tile_begin) * kTileBytes;
-  const uint64_t launch_end = launch_start + uint64_t(p.ntiles) * kTileBytes;
-  const uint64_t scan_limit = p.len < launch_end ? p.len : launch_end;  // blocks at or beyond it are not this launch's
   constexpr bool kMin = (kMode == 2);
   const uint64_t out_base = cin.count;
   uint32_t full_phase = 0;
@@ -775,14 +793,15 @@ SJ_DEV void scan_role(Smem *S, const sj_tensor_map *tmap, const ScanParams &p, c
   // Tickets should be scanned in roughly the order they were taken (every element waits for ALL lower tickets): at
   // start-up the second ticket is therefore taken only once the first block has arrived, when every CTA of the launch
   // has drawn its first one.
-  if (warp == 0) publish_ticket(S, 0, first_ticket, lane);  // (thread 0 drew it at the top of the kernel)
+  if (warp == 0) publish_ticket(S, 0, first_ticket, 0, lane);  // (thread 0 drew it at the top of the kernel)
   uint32_t t = wait_ticket(S, 0, p);
-  if (t < nelem) tma_cur = issue_load(S, tmap, p, t, warp, lane, 0, &pw_cur, scan_limit);
+  uint32_t fenced = 0xFFFFFFFFu;
+  if (t < nelem) tma_cur = issue_load(S, S->tdoc[0], p, t - S->doc[S->tdoc[0]].first_elem, warp, lane, 0, &pw_cur, &fenced);
   if (warp == 0) {
     if (tma_cur) wait_bar(&S->full[0][0], 0u, p, 32);
     uint32_t a1 = 0;
     if (lane == 0) a1 = sj_atomic_add(p.ticket, 1u);
-    publish_ticket(S, 1, a1, lane);
+    publish_ticket(S, 1, a1, S->tdoc[0], lane);
   }
   uint32_t ne = 0;  // this CTA's next element to emit (elements are emitted in order)
   uint32_t j = 0;
@@ -800,41 +819,45 @@ SJ_DEV void scan_role(Smem *S, const sj_tensor_map *tmap, const ScanParams &p, c
       // ticket j + 1 has been seen: a CTA's tickets must increase with j (the loops stop at the first one beyond the end).
       uint32_t a = 0;
       if (lane == 0) a = sj_atomic_add(p.ticket, 1u);
-      publish_ticket(S, j + 2, a, lane);
+      publish_ticket(S, j + 2, a, S->tdoc[(j + 1) % kNS], lane);
     }
     SJ_TRACE4(1);
-    if (tn < nelem) tma_next = issue_load(S, tmap, p, tn, warp, lane, r ^ 1, &pw_next, scan_limit);
+    if (tn < nelem) {
+      const uint32_t dn = S->tdoc[(j + 1) % kNS];
+      tma_next = issue_load(S, dn, p, tn - S->doc[dn].first_elem, warp, lane, r ^ 1, &pw_next, &fenced);
+    }
     SJ_TRACE4(2);
     uint8_t *T = S->ring[warp][r];
-    const uint64_t bstart = launch_start + uint64_t(t) * kElemBytes + uint64_t(warp) * kBlockBytes;
+    const DocEntry &D = S->doc[S->tdoc[j % kNS]];
+    const uint64_t bstart = launch_start + uint64_t(t - D.first_elem) * kElemBytes + uint64_t(warp) * kBlockBytes;
     if (!SJB200_SCAN4_TRACE && p.debug != nullptr && warp == 0 && lane == 0) {
       p.debug[uint64_t(t) * 8 + 0] = sj_globaltimer();
       p.debug[uint64_t(t) * 8 + 7] = ((unsigned long long)sj_smid() << 48) | ((unsigned long long)sj_cta() << 32) | j;
     }
     uint32_t summary = 0;
-    if (bstart < scan_limit) {
+    if (bstart < D.scan_end) {
       if (tma_cur) {
         wait_bar(&S->full[warp][r], (full_phase >> r) & 1u, p, 32);
         full_phase ^= 1u << r;
       } else {
-        fill_block_guarded(T, p, bstart, lane);
+        fill_block_guarded(T, D.buf, D.len, bstart, lane);
         sj_syncwarp();
       }
       SJ_TRACE4(3);
       const uint32_t pw0 = sj_shfl(pw_cur, 0);
-      const uint32_t st = boundary_state(p, bstart, launch_start, cin.state, pw0, lane);
+      const uint32_t st = boundary_state(D.buf, bstart, launch_start, cin.state, pw0, lane);
       SJ_TRACE4(4);
       {
         // the parked masks of element j - kParkFree must have been emitted before this element's take their place
         if (kEmitW && j >= uint32_t(kParkFree)) wait_bar(&S->park_free[j % kParkFree], ((j / kParkFree) - 1u) & 1u, p, 64);
-        const uint64_t left = p.len - bstart;  // > 0: bytes of the block that exist
+        const uint64_t left = D.len - bstart;  // > 0: bytes of the block that exist
         const uint32_t valid = left < uint64_t(kBlockBytes) ? uint32_t(left) : uint32_t(kBlockBytes);
         if (kEmitW && kGPark > 0) {
           uint32_t *slot = park_slot(p, j);
-          summary = scan_block<kMin>(T, pw0, st & 1u, (st >> 2) & 1u, lane, p, reinterpret_cast<sj_u4 *>(slot), reinterpret_cast<sj_u4 *>(slot) + kScanWarps * 32,
+          summary = scan_block<kMin>(T, pw0, st & 1u, (st >> 2) & 1u, lane, D.flags, reinterpret_cast<sj_u4 *>(slot), reinterpret_cast<sj_u4 *>(slot) + kScanWarps * 32,
                                      slot + 2 * kScanWarps * 32 * 4, valid);
         } else {
-          summary = scan_block<kMin>(T, pw0, st & 1u, (st >> 2) & 1u, lane, p, S->park[j % kPark][0], S->park[j % kPark][1], S->parkpre[j % kPark], valid);
+          summary = scan_block<kMin>(T, pw0, st & 1u, (st >> 2) & 1u, lane, D.flags, S->park[j % kPark][0], S->park[j % kPark][1], S->parkpre[j % kPark], valid);
         }
       }
     }
@@ -855,7 +878,7 @@ SJ_DEV void scan_role(Smem *S, const sj_tensor_map *tmap, const ScanParams &p, c
       if (sj_shfl(last, 0)) {
         sj_fence_block();
         if (!SJB200_SCAN4_TRACE && p.debug != nullptr && lane == 0) p.debug[uint64_t(t) * 8 + 3] = sj_globaltimer();
-        compose_element(S, p, ns, t, lane);
+        compose_element(S, p, ns, t, D.first_elem, lane);
         if (lane == 0) {
           S->arrived[ns] = 0;
           sj_mbar_arrive(&S->scanned[ns]);
@@ -969,7 +992,10 @@ SJ_DEV void emit_role(Smem *S, const sj_tensor_map *tmap, const ScanParams &p, c
 // The window is complete when everything newer than the nearest inclusive prefix has arrived.  Folding uses the fact
 // that only one bit is order-dependent: the quote parities of a group of 32 elements are one ballot word, an element's
 // polarity relative to the oldest element of the window is a popcount, and the counts are then plain sums.
-SJ_DEV void look_back(const ScanParams &p, uint32_t t, unsigned lane, uint32_t *s_in, uint32_t *base) {
+// doc_first: the first element of t's document.  The window never reaches below it: the previous document's descriptors
+// carry the same epoch, and its inclusive prefixes would give a wrong base.  (A document's first element publishes
+// only an inclusive prefix, so the nearest one is never older than it; the clamp also saves loading what lies beyond.)
+SJ_DEV void look_back(const ScanParams &p, uint32_t t, unsigned lane, uint32_t *s_in, uint32_t *base, uint32_t doc_first = 0) {
   Eff acc;
   acc.p = 0; acc.a = 0; acc.b = 0;
   int64_t newest = int64_t(t) - 1;
@@ -981,7 +1007,7 @@ SJ_DEV void look_back(const ScanParams &p, uint32_t t, unsigned lane, uint32_t *
 #pragma unroll
     for (int k = 0; k < kLookK; k++) {
       d[k] = 0;
-      if (first - 32 * k >= 0) pend |= 1u << k;
+      if (first - 32 * k >= int64_t(doc_first)) pend |= 1u << k;
     }
     const uint32_t want = pend;
     uint32_t inc_dist = 0xFFFFFFFFu, needed = (1u << kLookK) - 1u;
@@ -1050,7 +1076,7 @@ SJ_DEV void look_back(const ScanParams &p, uint32_t t, unsigned lane, uint32_t *
       return;
     }
     newest -= 32 * kLookK;
-    if (newest < 0) {  // cannot happen (element 0 always publishes an inclusive prefix); never loop forever
+    if (newest < int64_t(doc_first)) {  // cannot happen (a document's first element always publishes an inclusive prefix); never loop forever
       sj_atomic_or(p.flags, kFlagInternal);
       *s_in = acc.p;
       *base = acc.a;
@@ -1061,19 +1087,19 @@ SJ_DEV void look_back(const ScanParams &p, uint32_t t, unsigned lane, uint32_t *
 
 // The launch is over: total count, outgoing scanner state, the 6-bit carry transducer of everything it scanned
 // (multi-GPU shards fold these: SURVEY.md 8e), sentinels, end-of-input UTF-8 rule.
-SJ_DEV void finalize_launch(const ScanParams &p, const Carry &cin, uint32_t s_out, uint64_t count_total, unsigned lane) {
+// A multi-document launch finalises each document when its last element is resolved.
+SJ_DEV void finalize_launch(const ScanParams &p, const DocEntry &D, const Carry &cin, uint32_t s_out, uint64_t count_total, unsigned lane) {
   const uint64_t launch_start = uint64_t(p.tile_begin) * kTileBytes;
-  const uint64_t end_scanned = launch_start + uint64_t(p.ntiles) * kTileBytes;
-  const uint64_t end_real = p.len < end_scanned ? p.len : end_scanned;
+  const uint64_t end_real = D.scan_end;
   // state after the last real byte, for the carry-in this launch actually had
-  const uint32_t st = boundary_state(p, end_real, launch_start, cin.state, word_before(p, end_real), lane);
+  const uint32_t st = boundary_state(D.buf, end_real, launch_start, cin.state, word_before(D.buf, p.prev_word, end_real), lane);
   const uint32_t e_a = st & 1u, c_a = (st >> 2) & 1u, par_a = (s_out ^ (cin.state >> 1)) & 1u;
   // ... and for the opposite incoming escape: it can only toggle the first byte that is not a backslash
-  const uint64_t nlead = run_forward(p.buf, launch_start, end_real, lane);
+  const uint64_t nlead = run_forward(D.buf, launch_start, end_real, lane);
   uint32_t e_o = e_a, c_o = c_a, par_o = par_a;
   if (launch_start + nlead >= end_real) {
     e_o ^= 1u;  // nothing but backslashes: the carry goes straight through
-  } else if (sj_ldg_u8(p.buf + launch_start + nlead) == 0x22u) {
+  } else if (sj_ldg_u8(D.buf + launch_start + nlead) == 0x22u) {
     par_o ^= 1u;
     if (launch_start + nlead == end_real - 1) c_o ^= 1u;
   }
@@ -1081,38 +1107,39 @@ SJ_DEV void finalize_launch(const ScanParams &p, const Carry &cin, uint32_t s_ou
   const uint32_t T0 = ein ? (e_o | (par_o << 1) | (c_o << 2)) : (e_a | (par_a << 1) | (c_a << 2));
   const uint32_t T1 = ein ? (e_a | (par_a << 1) | (c_a << 2)) : (e_o | (par_o << 1) | (c_o << 2));
   if (lane == 0) {
-    p.carry_out->count = count_total;
-    p.carry_out->state = e_a | (s_out << 1) | (c_a << 2);
-    p.carry_out->ttable = T0 | (T1 << 3);
-    if (p.carry_out_host != nullptr) {
-      p.carry_out_host->count = count_total;
-      p.carry_out_host->state = e_a | (s_out << 1) | (c_a << 2);
-      p.carry_out_host->ttable = T0 | (T1 << 3);
+    D.carry_out->count = count_total;
+    D.carry_out->state = e_a | (s_out << 1) | (c_a << 2);
+    D.carry_out->ttable = T0 | (T1 << 3);
+    if (D.carry_out_host != nullptr) {
+      D.carry_out_host->count = count_total;
+      D.carry_out_host->state = e_a | (s_out << 1) | (c_a << 2);
+      D.carry_out_host->ttable = T0 | (T1 << 3);
     }
     if (p.write_sentinels) {  // json_structural_indexer.h L284-286
-      uint32_t *tail = p.idx_out + count_total;
-      tail[0] = uint32_t(p.len);
-      tail[1] = uint32_t(p.len);
+      uint32_t *tail = D.idx_out + count_total;
+      tail[0] = D.len;
+      tail[1] = D.len;
       tail[2] = 0;
     }
     if (p.check_eof) {  // utf8_checker::check_eof (utf8_lookup4_algorithm.h L167-171)
-      const uint32_t tw = word_before(p, p.len);
-      if (utf8_carry_pending(utf8_carry_from_prev_word(tw))) sj_atomic_or(p.flags, kFlagUtf8);
+      const uint32_t tw = word_before(D.buf, p.prev_word, D.len);
+      if (utf8_carry_pending(utf8_carry_from_prev_word(tw))) sj_atomic_or(D.flags, kFlagUtf8);
     }
   }
 }
 
 SJ_DEV void chain_role(Smem *S, const ScanParams &p, const Carry &cin, unsigned lane, unsigned c) {
-  const uint32_t nelem = elements_of(p);
+  const uint32_t nelem = launch_elements(S);
   for (uint32_t j = c;; j += uint32_t(kChainWarps)) {
     const int ns = int(j % kNS);
     const uint32_t t = wait_ticket(S, j, p);
     if (t >= nelem) break;
+    const DocEntry &D = S->doc[S->tdoc[ns]];
     uint32_t s_in = (cin.state >> 1) & 1u, base = 0;
     // The look-back needs the elements BEFORE t, not t itself: it runs while this CTA is still scanning t, so that the
     // element is resolved as soon as its own summary is there (with the look-back after the scan, an element waited
     // after the last of its predecessors had been scanned for the pick-up, the poll round trips and the fold).
-    if (t > 0) look_back(p, t, lane, &s_in, &base);
+    if (t > D.first_elem) look_back(p, t, lane, &s_in, &base, D.first_elem);
     wait_bar(&S->scanned[ns], (j / kNS) & 1u, p, 64);
     if (!SJB200_SCAN4_TRACE && p.debug != nullptr && lane == 0) p.debug[uint64_t(t) * 8 + 6] = sj_globaltimer();
     const uint32_t par = S->elem[ns][0], b0 = S->elem[ns][1], b1 = S->elem[ns][2], hits = S->elem[ns][3];
@@ -1125,11 +1152,11 @@ SJ_DEV void chain_role(Smem *S, const ScanParams &p, const Carry &cin, unsigned 
       S->res_base[ns][lane] = base + (pk & 0x7FFFFFFFu);
     }
     const uint32_t hit0 = hits & 1u, hit1 = (hits >> 1) & 1u;
-    if (lane == 0 && (s_in ? hit1 : hit0)) sj_atomic_or(p.flags, kFlagCtl);
+    if (lane == 0 && (s_in ? hit1 : hit0)) sj_atomic_or(D.flags, kFlagCtl);
     sj_syncwarp();
     if (lane == 0) sj_mbar_arrive(&S->resolved[ns]);
     if (!SJB200_SCAN4_TRACE && p.debug != nullptr && lane == 0) p.debug[uint64_t(t) * 8 + 4] = sj_globaltimer();
-    if (t == nelem - 1) finalize_launch(p, cin, s_out, cin.count + base + mine_total, lane);
+    if (t == D.first_elem + D.nelem - 1) finalize_launch(p, D, cin, s_out, cin.count + base + mine_total, lane);
   }
 }
 
@@ -1174,6 +1201,26 @@ SJ_DEV void scan4_body(const sj_tensor_map *tmap, const ScanParams &p, uint8_t *
   }
   if (tid < unsigned(kNS + 2 * kScanWarps + kParkFree + (kEmitWarps > 0 ? kEmitWarps : 1))) sj_fence_mbar_init();
   if (kMode == 2 && tid < 16) S->compact_lut[tid] = compact_entry(tid);
+  if (p.ndocs > 0) {  // the document table, 16 bytes per thread
+    const uint32_t nw = p.ndocs * uint32_t(sizeof(DocEntry) / 16);
+    for (uint32_t i = tid; i < nw; i += unsigned(kThreads4))
+      reinterpret_cast<sj_u4 *>(S->doc)[i] = sj_ldg_u4(reinterpret_cast<const uint8_t *>(p.docs) + 16 * size_t(i));
+    if (tid == 0) S->ndocs = p.ndocs;
+  } else if (tid == 0) {
+    DocEntry &D = S->doc[0];
+    const uint64_t launch_end = (uint64_t(p.tile_begin) + p.ntiles) * kTileBytes;
+    D.buf = p.buf;
+    D.idx_out = p.idx_out;
+    D.carry_out = p.carry_out;
+    D.carry_out_host = p.carry_out_host;
+    D.flags = p.flags;
+    D.tmap = p.use_tma ? static_cast<const void *>(tmap) : nullptr;
+    D.len = uint32_t(p.len);
+    D.scan_end = uint32_t(p.len < launch_end ? p.len : launch_end);
+    D.first_elem = 0;
+    D.nelem = elements_of(p);
+    S->ndocs = 1;
+  }
   sj_syncthreads();
 #if SJB200_SCAN4_TRACE
   if (tid == 0) S->trace_cta[1] = sj_globaltimer();
@@ -1204,9 +1251,15 @@ SJ_DEV void scan4_body(const sj_tensor_map *tmap, const ScanParams &p, uint8_t *
       p.ticket[0] = 0;
       p.ticket[1] = 0;
       p.ticket[2] = 0;
-      const uint32_t fl = sj_atomic_exch(p.flags, 0u);
-      p.carry_out->flags = fl;
-      if (p.carry_out_host != nullptr) p.carry_out_host->flags = fl;
+      // every document gets its own flags and the launch's (a single-document launch has one word for both)
+      const uint32_t fl_launch = sj_atomic_exch(p.flags, 0u);
+      uint32_t fl = fl_launch;
+      for (uint32_t d = 0; d < S->ndocs; d++) {
+        const DocEntry &D = S->doc[d];
+        fl = fl_launch | (D.flags != p.flags ? sj_atomic_exch(D.flags, 0u) : 0u);
+        D.carry_out->flags = fl;
+        if (D.carry_out_host != nullptr) D.carry_out_host->flags = fl;
+      }
       if (p.xchg_nranks != 0) {
         // the exchange step of a sharded scan, fused: this launch's record goes straight into every rank's window
         // (finalize_launch's stores are visible here: its CTA fenced before it counted itself out)

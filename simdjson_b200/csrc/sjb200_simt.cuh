@@ -189,6 +189,7 @@ SJ_DEV void sj_mbar_init(sj_mbar_t *b, uint32_t count) {
 }
 SJ_DEV void sj_fence_mbar_init() {}
 SJ_DEV void sj_fence_proxy_async() {}
+SJ_DEV void sj_fence_tensormap_acquire(const void *) {}
 SJ_DEV void sj_mbar_arrive(sj_mbar_t *b) {
   std::lock_guard<std::mutex> g(b->mu);
   b->pending--;
@@ -324,6 +325,10 @@ SJ_DEV void sj_fence_mbar_init() { asm volatile("fence.mbarrier_init.release.clu
 // (MEMBAR.ALL.CTA + FENCE.VIEW.ASYNC: waits for the thread's outstanding loads -- issue it before, not after, a global
 // load whose value is not needed yet)
 SJ_DEV void sj_fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// a tensor map in global memory that the host wrote (cudaMemcpy) is used by this thread's TMA loads only after this fence
+SJ_DEV void sj_fence_tensormap_acquire(const void *map) {
+  asm volatile("fence.proxy.tensormap::generic.acquire.sys [%0], 128;" ::"l"(map) : "memory");
+}
 SJ_DEV void sj_mbar_arrive(sj_mbar_t *bar) {
   asm volatile("mbarrier.arrive.release.cta.shared::cta.b64 _, [%0];" ::"r"(sj_smem_u32(bar)) : "memory");
 }

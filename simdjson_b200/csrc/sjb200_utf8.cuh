@@ -103,7 +103,7 @@ SJ_DEV void utf8_body(const sj_tensor_map *tmap, const ScanParams &p, uint8_t *s
         sj_mbar_arrive_expect_tx(&S->full[warp][r], kBlockBytesU);
         sj_tma_load_rows(S->ring[warp][r], tmap, &S->full[warp][r], uint32_t(row));
       }
-      *pw = scan4::word_before(p, bstart);  // after the fence: it would wait for this load
+      *pw = scan4::word_before(p.buf, p.prev_word, bstart);  // after the fence: it would wait for this load
     }
     return full;
   };
@@ -127,7 +127,7 @@ SJ_DEV void utf8_body(const sj_tensor_map *tmap, const ScanParams &p, uint8_t *s
       scan4::wait_bar(&S->full[warp][r], (phase >> r) & 1u, p, 32);
       phase ^= 1u << r;
     } else {
-      scan4::fill_block_guarded(T, p, launch_start + b * kBlockBytesU, lane);
+      scan4::fill_block_guarded(T, p.buf, p.len, launch_start + b * kBlockBytesU, lane);
       sj_syncwarp();
     }
     err |= check_block(T, sj_shfl(pwq[0], 0), lane);
@@ -142,7 +142,7 @@ SJ_DEV void utf8_body(const sj_tensor_map *tmap, const ScanParams &p, uint8_t *s
     rn = (rn + 1 == uint32_t(kSlotsU)) ? 0u : rn + 1;
   }
   if (p.check_eof && g == 0 && lane == 0) {  // utf8_checker::check_eof (utf8_lookup4_algorithm.h L167-171): input must not end inside a sequence
-    if (utf8_carry_pending(utf8_carry_from_prev_word(scan4::word_before(p, p.len)))) err |= 1u;
+    if (utf8_carry_pending(utf8_carry_from_prev_word(scan4::word_before(p.buf, p.prev_word, p.len)))) err |= 1u;
   }
   if (sj_any(err != 0) && lane == 0) sj_atomic_or(p.flags, kFlagUtf8);
   // last CTA out hands the flags over and re-arms them (same protocol as the other scans of a context)
