@@ -198,6 +198,8 @@ def run_ndjson(args, rank, world, total=1 << 30):
 # =============================================================================== configs[3]: validate_utf8 + minify, 256 MiB
 def run_utf8_minify(args, rank, world, size=256 << 20):
     torch, dist, sj, dev, local = _setup(rank, world)
+    if world > 1:
+        return run_utf8_minify_sharded(args, rank, world, size)
     if rank != 0:
         return True
     from simdjson_b200 import corpus
@@ -248,6 +250,94 @@ def run_utf8_minify(args, rank, world, size=256 << 20):
                              "roofline": dict(_roofline(size + dl, mms, "scan4_minify_kernel"), kernel="sjb200::scan4_minify_kernel (1 B read + kept bytes written per input byte)")},
                   "e2e": {"value": None, "unit": B.UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0, "note": "device-resident configuration"}})
     print(json.dumps(line), flush=True)
+    parser.close()
+    return ok
+
+
+def _scan_state(port, buf):
+    """the oracle's scanner state after buf (bit0 escape, bit1 in string, bit2 previous byte scalar)"""
+    L = port.L
+    L.sjo_scan_shard.restype = C.c_uint64
+    L.sjo_scan_shard.argtypes = [C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)]
+    a = np.ascontiguousarray(buf, dtype=np.uint8)
+    so = C.c_uint32(0)
+    L.sjo_scan_shard(a.ctypes.data if len(a) else None, len(a), 0, None, C.byref(so))
+    return int(so.value)
+
+
+def run_utf8_minify_sharded(args, rank, world, size):
+    """configs[3] over N ranks: every rank validates its shard of the 256 MiB text (cut at character boundaries) and
+    minifies its shard of the 256 MiB pretty JSON (cut at the nominal byte: inside strings, escapes, characters), through
+    sjb200_validate_utf8_sharded / sjb200_minify_sharded.  Each pass is timed with CUDA events on its rank, from before
+    the enqueue to after the finish (the exchange and any second round included); a 256 MiB buffer is written between
+    passes (cold L2).  value = whole-buffer bytes / the slowest rank's mean pass."""
+    torch, dist, sj, dev, local = _setup(rank, world)
+    from simdjson_b200 import corpus, sharding
+    O = B.oracle()
+    port = O.Port()
+    steps = args.steps
+    u = corpus.random_utf8(size).copy()
+    ucuts = sharding.shard_cuts(u, world)
+    j = corpus.random_json(size, pretty_bias=0.8, utf8_rate=0.15).copy()
+    jcuts = [size * k // world for k in range(world + 1)]
+    ushard = np.ascontiguousarray(u[ucuts[rank]: ucuts[rank + 1]])
+    jshard = np.ascontiguousarray(j[jcuts[rank]: jcuts[rank + 1]])
+    rc, parser = sj.get_active_implementation(local).create_dom_parser_implementation(max(len(ushard), len(jshard)))
+    stream = torch.cuda.Stream(device=dev)
+    torch.cuda.set_stream(stream)
+    comm = _connect(torch, dist, sharding, parser, rank, world, dev)
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
+    du = torch.from_numpy(ushard).to(dev)
+    dj = torch.from_numpy(jshard).to(dev)
+    dst = torch.zeros(len(jshard), dtype=torch.uint8, device=dev)
+
+    def timed(one_pass):
+        ts, last = [], None
+        for it in range(steps + 1):  # the first pass is not timed
+            flush.fill_(it)
+            torch.cuda.synchronize()
+            dist.barrier()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record(stream)
+            last = one_pass()
+            e1.record(stream)
+            torch.cuda.synchronize()
+            ts.append(e0.elapsed_time(e1))
+        return _max_over_ranks(torch, dist, dev, world, float(np.mean(ts[1:]))), last
+    # ---- validate_utf8: the valid buffer, then a copy with one corrupted byte in the middle rank's shard
+    ums, (v, _) = timed(lambda: comm.validate_utf8(du, stream))
+    bad = du.clone()
+    if rank == world // 2:
+        bad[len(ushard) // 2] = 0xFF
+    vbad, _ = comm.validate_utf8(bad, stream)
+    del bad
+    ok = v == 1 and vbad == 0 and port.validate_utf8(u)
+    # ---- minify
+    mms, (rcm, res) = timed(lambda: comm.minify(dj, dst, stream))
+    werr, want = port.minify(j)
+    count, base = int(res.count), int(res.base)
+    okm = rcm == werr == 0 and int(res.total_count) == len(want) and bytes(dst[:count].cpu().numpy()) == want[base: base + count]
+    okm = okm and int(res.state_in) == _scan_state(port, j[: jcuts[rank]]) and int(res.rescanned) == (1 if res.state_in & 3 else 0)
+    info = torch.tensor([count, base, int(res.rescanned)], dtype=torch.int64, device=dev)
+    allinfo = torch.empty(3 * world, dtype=torch.int64, device=dev)
+    dist.all_gather_into_tensor(allinfo, info)
+    allinfo = allinfo.view(world, 3).cpu().numpy()
+    okm = okm and all(int(allinfo[r, 1]) == int(allinfo[:r, 0].sum()) for r in range(world))
+    ok = _all_ok(torch, dist, dev, world, bool(ok and okm))
+    if rank == 0:
+        line = _line(args, world, size / (ums * 1e-3) / 1e9, ums,
+                     {"workload": f"validate_utf8 + minify on 256 MiB mixed-ASCII/UTF-8 synthetic, sharded by byte range over {world}xH100 (BASELINE.json configs[3])",
+                      "bytes": size, "l2": "a 256 MiB buffer is written between passes (cold L2)",
+                      "value_is": "validate_utf8 input GB/s of the whole buffer (slowest rank's mean pass, exchange included); minify below",
+                      "cuts": "validate_utf8: character boundaries (sjb200_shard_cut); minify: nominal bytes",
+                      "api": "sjb200_validate_utf8_sharded / sjb200_minify_sharded (exchange fused into the kernels)"},
+                     {"parity": {"ok": ok, "against": "CPU oracle: verdict (valid + 1 corrupted copy) on every rank; every rank's kept bytes at its base in the whole buffer's minify"},
+                      "gpu_launches": 2 * (steps + 1) + 1,
+                      "minify": {"input_gbs": round(size / (mms * 1e-3) / 1e9, 1), "ms": round(mms, 5), "kept_fraction": round(len(want) / size, 4),
+                                 "rescans": int(allinfo[:, 2].sum())},
+                      "e2e": {"value": None, "unit": B.UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0, "note": "device-resident configuration"}})
+        print(json.dumps(line), flush=True)
+    comm.close()
     parser.close()
     return ok
 
@@ -389,8 +479,10 @@ def run_concat(args, rank, world, nshards=8, shard_target=1 << 30):
 def run_check(args, rank, world, total=256 << 20):
     """ONE NDJSON buffer cut at arbitrary character boundaries (mid-row, mid-string): carry-in != 0, wrong speculations,
     second exchange round and re-scans, through the real plumbing (CUDA IPC windows; NCCL for the handles).  Every rank
-    compares its base + indexes with the oracle's scan of the whole prefix.  With one process (no torchrun) the ranks run
-    as threads of this process on one GPU."""
+    compares its base + indexes with the oracle's scan of the whole prefix.  Then sharded minify on the same buffer and
+    cuts (every rank's kept bytes at its base in the oracle's minify of the whole buffer) and sharded validate_utf8 on
+    random UTF-8 cut at character boundaries, valid and with one corrupted byte: one JSON line each.  With one process
+    (no torchrun) the ranks run as threads of this process on one GPU."""
     torch, dist, sj, dev, local = _setup(rank, world)
     from simdjson_b200 import corpus, sharding
     O = B.oracle()
@@ -415,6 +507,7 @@ def run_check(args, rank, world, total=256 << 20):
             pos = hit + 1
     del raw
     report = {"ranks": nranks, "bytes": total, "cuts": "character boundaries (sjb200_shard_cut), every odd cut moved inside a string value", "processes": world}
+    states = [0] + [_scan_state(port, doc[: cuts[r]]) for r in range(1, nranks)]  # true incoming state of every shard
 
     def verify(r, res, got):
         want_all, state_before = B.raw_scan(O, port, doc[: cuts[r]], 0) if r else (np.zeros(0, np.uint32), 0)
@@ -422,50 +515,102 @@ def run_check(args, rank, world, total=256 << 20):
         return (res.state_in == state_before and res.base == len(want_all) and res.count == len(widx) and np.array_equal(got[: res.count], widx)
                 and res.rescanned == (1 if state_before else 0)), int(res.rescanned), int(state_before)
 
-    if world > 1:
-        rc, parser = sj.get_active_implementation(local).create_dom_parser_implementation(cuts[rank + 1] - cuts[rank])
-        comm = _connect(torch, dist, sharding, parser, rank, world, dev)
-        d = torch.from_numpy(np.ascontiguousarray(doc[cuts[rank]: cuts[rank + 1]])).to(dev)
+    def stage1_body(r, comm, parser, d, stream):
         d_idx = torch.empty(int(sj.lib().sjb200_index_words(d.numel())), dtype=torch.int32, device=dev)
-        rcs, res = comm.scan(d, d_idx, rank == world - 1)
+        rcs, res = comm.scan(d, d_idx, r == nranks - 1, stream)
         torch.cuda.synchronize()
-        ok, resc, st = verify(rank, res, d_idx.cpu().numpy().view(np.uint32)) if rcs == 0 else (False, 0, 0)
-        info = torch.tensor([resc, st], dtype=torch.int64, device=dev)
-        allinfo = torch.empty(2 * world, dtype=torch.int64, device=dev)
-        dist.all_gather_into_tensor(allinfo, info)
-        ok = _all_ok(torch, dist, dev, world, ok)
-        report.update({"rescans": int(allinfo.view(world, 2)[:, 0].sum().item()), "states_in": [int(x) for x in allinfo.view(world, 2)[:, 1].cpu()]})
-        comm.close()
-        parser.close()
-    else:
-        parsers, comms = [], []
-        for r in range(nranks):
-            rc, p = sj.get_active_implementation(local).create_dom_parser_implementation(cuts[r + 1] - cuts[r])
-            parsers.append(p)
-            comms.append(sharding.Comm(p, r, nranks))
-        sharding.Comm.connect_local(comms)
-        outs = [None] * nranks
+        return verify(r, res, d_idx.cpu().numpy().view(np.uint32)) if rcs == 0 else (False, 0, 0)
 
-        def work(r):
-            torch.cuda.set_device(local)
-            d = torch.from_numpy(np.ascontiguousarray(doc[cuts[r]: cuts[r + 1]])).to(dev)
-            d_idx = torch.empty(int(sj.lib().sjb200_index_words(d.numel())), dtype=torch.int32, device=dev)
-            rcs, res = comms[r].scan(d, d_idx, r == nranks - 1, torch.cuda.Stream(device=dev))
-            torch.cuda.synchronize()
-            outs[r] = verify(r, res, d_idx.cpu().numpy().view(np.uint32)) if rcs == 0 else (False, 0, 0)
-        th = [threading.Thread(target=work, args=(r,)) for r in range(nranks)]
-        [t.start() for t in th]
-        [t.join() for t in th]
-        ok = all(o is not None and o[0] for o in outs)
-        report.update({"rescans": sum(o[1] for o in outs if o), "states_in": [o[2] for o in outs if o]})
-        for c in comms:
-            c.close()
-        for p in parsers:
-            p.close()
+    ok, infos = _sharded_ranks(torch, dist, sj, sharding, dev, local, rank, world, nranks, lambda r: doc[cuts[r]: cuts[r + 1]], stage1_body)
+    report.update({"rescans": sum(i[1] for i in infos), "states_in": [i[2] for i in infos]})
     if rank == 0:
         report["ok"] = bool(ok)
         print(json.dumps({"check": "sharded stage 1, carry-in != 0 (BASELINE.json configs[2] cut mid-row)", "result": report}), flush=True)
-    return ok
+
+    # ---- minify on the same cuts: the ranks behind an odd cut start inside a string, minify again from their true state
+    werr, want = port.minify(doc)
+
+    def minify_body(r, comm, parser, d, stream):
+        dst = torch.empty(d.numel(), dtype=torch.uint8, device=dev)
+        rcs, res = comm.minify(d, dst, stream)
+        torch.cuda.synchronize()
+        if rcs != 0 or werr != 0:
+            return (False, 0, 0, 0, 0)
+        base, count = int(res.base), int(res.count)
+        good = (bytes(dst[:count].cpu().numpy()) == want[base: base + count] and int(res.total_count) == len(want) and res.state_in == states[r]
+                and res.rescanned == (1 if states[r] & 3 else 0))
+        return good, int(res.rescanned), int(res.state_in), count, base
+
+    ok_m, infos = _sharded_ranks(torch, dist, sj, sharding, dev, local, rank, world, nranks, lambda r: doc[cuts[r]: cuts[r + 1]], minify_body)
+    ok_m = ok_m and all(infos[r][4] == sum(i[3] for i in infos[:r]) for r in range(nranks))  # bases are the prefix sums of the counts
+    if rank == 0:
+        print(json.dumps({"check": "sharded minify, carry-in != 0 (the same buffer and cuts)",
+                          "result": {"ranks": nranks, "bytes": total, "cuts": report["cuts"], "processes": world, "minified_bytes": len(want),
+                                     "rescans": sum(i[1] for i in infos), "states_in": [i[2] for i in infos], "ok": bool(ok_m)}}), flush=True)
+
+    # ---- validate_utf8: random UTF-8 cut at character boundaries, then a copy with one corrupted byte in one shard
+    text = corpus.random_utf8(total // 4).copy()
+    tcuts = sharding.shard_cuts(text, nranks)
+    bad = text.copy()
+    bad[(tcuts[nranks // 2] + tcuts[nranks // 2 + 1]) // 2] = 0xFF
+    verdicts = []
+    ok_u = True
+    for buf, want_v in ((text, 1), (bad, 0)):
+        assert port.validate_utf8(buf) == bool(want_v)
+
+        def utf8_body(r, comm, parser, d, stream, want_v=want_v):
+            v, res = comm.validate_utf8(d, stream)
+            torch.cuda.synchronize()
+            return v == want_v and res.rescanned == 0, v
+
+        good, infos = _sharded_ranks(torch, dist, sj, sharding, dev, local, rank, world, nranks, lambda r, buf=buf: buf[tcuts[r]: tcuts[r + 1]], utf8_body)
+        ok_u = ok_u and good
+        verdicts.append([i[1] for i in infos])
+    if rank == 0:
+        print(json.dumps({"check": "sharded validate_utf8, AND of the shards' verdicts",
+                          "result": {"ranks": nranks, "bytes": len(text), "cuts": "character boundaries (sjb200_shard_cut)", "processes": world,
+                                     "verdicts": {"valid": verdicts[0], "one corrupted byte": verdicts[1]}, "ok": bool(ok_u)}}), flush=True)
+    return bool(ok and ok_m and ok_u)
+
+
+def _sharded_ranks(torch, dist, sj, sharding, dev, local, rank, world, nranks, shard_of, body):
+    """body(r, comm, parser, d_shard, stream) -> (ok, int, ...) for every rank of a sharded check: this process's rank
+    under torchrun (one process per GPU, CUDA IPC windows), else all nranks ranks as threads of this process on one GPU
+    (connect_local).  Returns (ok on every rank, every rank's tuple, by rank)."""
+    if world > 1:
+        shard = np.ascontiguousarray(shard_of(rank))
+        rc, parser = sj.get_active_implementation(local).create_dom_parser_implementation(len(shard))
+        comm = _connect(torch, dist, sharding, parser, rank, world, dev)
+        d = torch.from_numpy(shard).to(dev)
+        mine = body(rank, comm, parser, d, None)
+        info = torch.tensor([int(x) for x in mine], dtype=torch.int64, device=dev)
+        allinfo = torch.empty(world * len(mine), dtype=torch.int64, device=dev)
+        dist.all_gather_into_tensor(allinfo, info)
+        comm.close()
+        parser.close()
+        infos = [tuple(int(x) for x in row) for row in allinfo.view(world, len(mine)).cpu().numpy()]
+        return _all_ok(torch, dist, dev, world, bool(mine[0])), infos
+    parsers, comms = [], []
+    for r in range(nranks):
+        rc, p = sj.get_active_implementation(local).create_dom_parser_implementation(len(shard_of(r)))
+        parsers.append(p)
+        comms.append(sharding.Comm(p, r, nranks))
+    sharding.Comm.connect_local(comms)
+    outs = [None] * nranks
+
+    def work(r):
+        torch.cuda.set_device(local)
+        d = torch.from_numpy(np.ascontiguousarray(shard_of(r))).to(dev)
+        outs[r] = body(r, comms[r], parsers[r], d, torch.cuda.Stream(device=dev))
+    th = [threading.Thread(target=work, args=(r,)) for r in range(nranks)]
+    [t.start() for t in th]
+    [t.join() for t in th]
+    for c in comms:
+        c.close()
+    for p in parsers:
+        p.close()
+    ok = all(o is not None and o[0] for o in outs)
+    return ok, [tuple(int(x) for x in o) if o is not None else (0,) * 5 for o in outs]
 
 
 def run(args, rank, world):

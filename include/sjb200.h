@@ -24,7 +24,8 @@
  *   sjb200_validate_utf8
  *        implementation::validate_utf8(buf,len)              include/simdjson/implementation.h L128
  * The *_dev variants take device pointers (input already resident in HBM); they are what the
- * roofline metric times.  The sharded variant is the per-GPU piece of a multi-GPU scan (section 8e).
+ * roofline metric times.  The sharded variants (stage 1, minify, validate_utf8) are the per-GPU pieces of a multi-GPU
+ * pass over one buffer cut by byte range (section 8e).
  */
 #ifndef SJB200_H
 #define SJB200_H
@@ -216,14 +217,14 @@ SJB200_API int sjb200_stage1_shard_dev_enqueue(sjb200_ctx *ctx, const uint8_t *d
  * One sjb200_comm per rank (one process per GPU, or several contexts in one process).  Each comm owns an exchange
  * window in its device's memory; peers map each other's windows (CUDA IPC across processes: get_handle -> exchange the
  * 64-byte handles by any means, e.g. one NCCL/gloo all-gather at start-up -> connect).  During a pass the scan
- * kernel's last CTA stores the shard's 16-byte record {count, state, transducer, flags} straight into every rank's
+ * kernel's last CTA stores the shard's 16-byte record {count, state, transducer, flags, kind} straight into every rank's
  * window over NVLink; finish() folds the true incoming state / 64-bit index base from the local window and, only if
  * some rank's speculation (state 0) was wrong, re-scans that rank and runs a second round.  Indexes stay
  * shard-relative (uint32) + base, like document_stream's batch_start + structural_indexes[i]
  * (include/simdjson/dom/document_stream-inl.h L250).  Up to 32 passes may be in flight per rank. */
 typedef struct sjb200_comm sjb200_comm;
 #define SJB200_COMM_HANDLE_BYTES 64
-typedef struct {
+typedef struct {        /* counts are structurals (stage 1), kept bytes (minify) or 0 (validate_utf8) */
   uint64_t count;        /* structurals of this shard (after a re-scan: the corrected count) */
   uint64_t base;         /* structurals of all earlier shards: global index i of this shard = base + i */
   uint64_t total_count;  /* structurals of all shards */
@@ -244,6 +245,31 @@ SJB200_API int sjb200_stage1_sharded(sjb200_comm *comm, const uint8_t *d_shard, 
 SJB200_API int sjb200_stage1_sharded_enqueue(sjb200_comm *comm, const uint8_t *d_shard, size_t len, int last_shard, uint32_t *d_idx,
                                   void *stream);
 SJB200_API int sjb200_stage1_sharded_finish(sjb200_comm *comm, sjb200_sharded_result *out); /* completes the oldest pass in flight */
+
+/* minify and validate_utf8 sharded the same way, on the same comm and window.  A pass is stage 1, minify or
+ * validate_utf8 (its kind, carried in the record); passes of all kinds may be in flight together, up to the limit above,
+ * when every rank enqueues the same sequence of kinds.  Each finish completes the oldest pass in flight, which must be
+ * of its kind (else UNEXPECTED_ERROR and the pass stays in flight); a peer that published another kind for the same
+ * pass makes finish fail with UNEXPECTED_ERROR (validate: -1) and sets sjb200_last_cuda_error.  len >= 1.
+ *
+ * minify: d_dst needs len bytes; this shard's kept bytes are d_dst[0, out->count).  out->base = their offset in the
+ *   minified document, out->total_count = its length; state_in / final_state / flags / flags_all / rescanned as for stage
+ *   1, except that minify validates nothing, so only the internal-error bit of the flags is ever set.  Cuts may be at any byte (minify does not look at UTF-8; escape and in-string cross the cut in the state).  Only
+ *   bits 0-1 of the state change which bytes are kept, so a rank re-minifies only when (state_in & 3) != 0, and the second
+ *   round runs only when that holds for some rank.  When final_state bit 1 is set (the document ends inside a string)
+ *   every rank returns UNCLOSED_STRING, like sjb200_minify_dev, with `out` filled.  The outputs stay on their ranks:
+ *   gathering them is one copy of d_dst[0, count) to [base, base + count) per rank, by the caller.
+ * validate_utf8: finish returns 1 when every shard is valid UTF-8, 0 when one is not, negative on a CUDA failure or an
+ *   exchange timeout.  Cuts must be at character boundaries (sjb200_shard_cut), as for stage 1: then every shard checks
+ *   its own end and the AND of the shards' verdicts is the verdict on the whole buffer.  The records carry count 0,
+ *   state 0 and transducer 0, so no second round ever runs. */
+SJB200_API int sjb200_minify_sharded_enqueue(sjb200_comm *comm, const uint8_t *d_shard, size_t len, uint8_t *d_dst, void *stream);
+SJB200_API int sjb200_minify_sharded_finish(sjb200_comm *comm, sjb200_sharded_result *out);
+SJB200_API int sjb200_minify_sharded(sjb200_comm *comm, const uint8_t *d_shard, size_t len, uint8_t *d_dst, sjb200_sharded_result *out,
+                          void *stream);
+SJB200_API int sjb200_validate_utf8_sharded_enqueue(sjb200_comm *comm, const uint8_t *d_shard, size_t len, void *stream);
+SJB200_API int sjb200_validate_utf8_sharded_finish(sjb200_comm *comm, sjb200_sharded_result *out);
+SJB200_API int sjb200_validate_utf8_sharded(sjb200_comm *comm, const uint8_t *d_shard, size_t len, sjb200_sharded_result *out, void *stream);
 
 /* fold: state entering shard r given the ttables of shards 0..r-1 and the document's initial state 0 */
 SJB200_API uint32_t sjb200_fold_state(const uint32_t *ttables, int nshards_before);

@@ -20,6 +20,8 @@ EXPORTS = [
     "sjb200_stage1_shard_dev", "sjb200_stage1_shard_dev_enqueue", "sjb200_fold_state", "sjb200_shard_cut", "sjb200_shard_cut_line",
     "sjb200_comm_create", "sjb200_comm_destroy", "sjb200_comm_get_handle", "sjb200_comm_connect", "sjb200_comm_connect_local",
     "sjb200_stage1_sharded", "sjb200_stage1_sharded_enqueue", "sjb200_stage1_sharded_finish",
+    "sjb200_minify_sharded", "sjb200_minify_sharded_enqueue", "sjb200_minify_sharded_finish",
+    "sjb200_validate_utf8_sharded", "sjb200_validate_utf8_sharded_enqueue", "sjb200_validate_utf8_sharded_finish",
     "sjb200_tokens_dev", "sjb200_string_buf_capacity",
 ]
 COMM_HANDLE_BYTES = 64
@@ -98,6 +100,12 @@ def load():
         "sjb200_stage1_sharded": (C.c_int, [vp, vp, sz, C.c_int, vp, C.POINTER(ShardedResult), vp]),
         "sjb200_stage1_sharded_enqueue": (C.c_int, [vp, vp, sz, C.c_int, vp, vp]),
         "sjb200_stage1_sharded_finish": (C.c_int, [vp, C.POINTER(ShardedResult)]),
+        "sjb200_minify_sharded": (C.c_int, [vp, vp, sz, vp, C.POINTER(ShardedResult), vp]),
+        "sjb200_minify_sharded_enqueue": (C.c_int, [vp, vp, sz, vp, vp]),
+        "sjb200_minify_sharded_finish": (C.c_int, [vp, C.POINTER(ShardedResult)]),
+        "sjb200_validate_utf8_sharded": (C.c_int, [vp, vp, sz, C.POINTER(ShardedResult), vp]),
+        "sjb200_validate_utf8_sharded_enqueue": (C.c_int, [vp, vp, sz, vp]),
+        "sjb200_validate_utf8_sharded_finish": (C.c_int, [vp, C.POINTER(ShardedResult)]),
         "sjb200_tokens_dev": (C.c_int, [vp, vp, sz, vp, C.c_uint32, vp, vp, vp, sz, C.POINTER(TokensResult), vp]),
         "sjb200_string_buf_capacity": (sz, [sz]),
     }

@@ -277,7 +277,7 @@ bool enqueue_scan(sjb200_ctx *c, int kind, const CUtensorMap *map, bool tma, con
   p.flags = c->d_flags;
   p.count_desc = c->d_count_desc;
   p.ticket = c->d_ticket;
-  if (xchg && use_scan4(c, kind)) {
+  if (xchg) {  // both kernels publish the record (scan4: stage 1 and minify; utf8v2: validate_utf8)
     for (int r = 0; r < kMaxRanks; r++) p.xchg_peer[r] = xchg->peer[r];
     p.xchg_nranks = xchg->nranks; p.xchg_rank = xchg->rank; p.xchg_slot = xchg->slot; p.xchg_seq = xchg->seq;
   }
@@ -1274,9 +1274,11 @@ extern "C" int sjb200_stage1_shard_dev_enqueue(sjb200_ctx *c, const uint8_t *d_b
 // One object per rank.  The exchange window lives in device memory; peers map it through CUDA IPC (one process per GPU,
 // the torch.distributed / MPI layout) or directly (several contexts in one process).  A pass = every rank scans its
 // shard with the speculated state 0; the scan kernel's last CTA stores the 16-byte record {count, state, transducer,
-// flags} into every rank's window over NVLink -- no collective launch.  finish() reads the local window, folds the
-// true incoming state and index base, and -- only when somebody's speculation was wrong -- re-scans and runs a second
-// round.  Up to kXchgSteps / 2 passes may be in flight per rank (enqueue ... enqueue, finish ... finish).
+// flags, kind} into every rank's window over NVLink -- no collective launch.  finish() reads the local window, folds the
+// true incoming state and base, and -- only when somebody's speculation was wrong -- re-scans and runs a second round.
+// A pass is stage 1, minify or validate_utf8 (its kind); passes of all kinds share the window and may be in flight
+// together, up to kXchgSteps / 2 per rank (enqueue ... enqueue, finish ... finish), as long as every rank enqueues the
+// same sequence of kinds.
 struct sjb200_comm {
   sjb200_ctx *ctx = nullptr;
   int rank = 0, nranks = 1;
@@ -1288,7 +1290,7 @@ struct sjb200_comm {
   Carry *d_result = nullptr;                       // [kXchgSteps] the launches' own result blocks
   cudaStream_t poll_stream = nullptr;
   cudaEvent_t done[kXchgSteps] = {};
-  struct Step { const uint8_t *d_buf; size_t len; uint32_t *d_idx; cudaStream_t stream; uint32_t seq; int last; } steps[kXchgSteps];
+  struct Step { const uint8_t *d_buf; size_t len; uint32_t *d_idx; uint8_t *d_dst; cudaStream_t stream; uint32_t seq; int last; int kind; } steps[kXchgSteps];
   uint32_t head = 0, tail = 0;                     // passes enqueued / finished
   long poll_timeout_ms = 20000;
 };
@@ -1400,53 +1402,88 @@ extern "C" int sjb200_comm_connect_local(sjb200_comm *m, sjb200_comm *const *all
   return SJB200_SUCCESS;
 }
 
-extern "C" int sjb200_stage1_sharded_enqueue(sjb200_comm *m, const uint8_t *d_shard, size_t len, int last_shard, uint32_t *d_idx, void *stream) {
-  if (!m || !m->connected || !d_shard || !d_idx || len == 0 || len > kMaxBytes) return SJB200_UNEXPECTED_ERROR;
+namespace {
+// Enqueue one pass of `kind` (kIndex: d_idx, kMinify: d_dst, kUtf8: neither).  The launch's record lands in every rank's
+// window; m->done[slot] marks the end of the launch on `stream`.
+int sharded_enqueue(sjb200_comm *m, int kind, const uint8_t *d_shard, size_t len, int last_shard, uint32_t *d_idx, uint8_t *d_dst, void *stream) {
+  if (!m || !m->connected || !d_shard || len == 0 || len > kMaxBytes || (kind == kIndex && !d_idx) || (kind == kMinify && !d_dst))
+    return SJB200_UNEXPECTED_ERROR;
   if (m->head - m->tail >= uint32_t(kXchgSteps / 2)) return SJB200_CAPACITY;  // too many passes in flight: finish some first
   sjb200_ctx *c = m->ctx;
-  if (!use_scan4(c, kIndex)) return SJB200_UNEXPECTED_ERROR;
   DeviceGuard g(c->device);
   const auto t_enq = std::chrono::steady_clock::now();
   cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
-  if (!ensure_desc(c, len)) return SJB200_MEMALLOC;
+  if (use_scan4(c, kind) && !ensure_desc(c, len)) return SJB200_MEMALLOC;
   const uint32_t seq = m->head + 1;  // tags start at 1: a zeroed window never matches
   XchgTarget x;
   for (int r = 0; r < kMaxRanks; r++) x.peer[r] = m->peer[r];
   x.nranks = uint32_t(m->nranks); x.rank = uint32_t(m->rank); x.slot = window_slot(seq, 0); x.seq = seq;
   CUtensorMap map;
   bool tma = false;
-  map_for(c, kIndex, &map, d_shard, len, &tma);
-  sjb200_comm::Step &st = m->steps[m->head % uint32_t(kXchgSteps)];
-  st.d_buf = d_shard; st.len = len; st.d_idx = d_idx; st.stream = s; st.seq = seq; st.last = last_shard;
-  if (!enqueue_scan(c, kIndex, &map, tma, d_shard, len, 0, tiles_of(len), true, 0x20202020u, d_idx, nullptr, -1, s, 1, false,
-                    m->d_result + (m->head % uint32_t(kXchgSteps)), nullptr, &x) ||
-      !ok(c, cudaEventRecord(m->done[m->head % uint32_t(kXchgSteps)], s), "event record"))
+  map_for(c, kind, &map, d_shard, len, &tma);
+  const uint32_t i = m->head % uint32_t(kXchgSteps);
+  sjb200_comm::Step &st = m->steps[i];
+  st.d_buf = d_shard; st.len = len; st.d_idx = d_idx; st.d_dst = d_dst; st.stream = s; st.seq = seq; st.last = last_shard; st.kind = kind;
+  if (!enqueue_scan(c, kind, &map, tma, d_shard, len, 0, tiles_of(len), true, 0x20202020u, d_idx, d_dst, -1, s, 1, false, m->d_result + i, nullptr, &x) ||
+      !ok(c, cudaEventRecord(m->done[i], s), "event record"))
     return SJB200_UNEXPECTED_ERROR;
   m->head++;
   c->xchg_enqueue_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_enq).count();
   return SJB200_SUCCESS;
 }
 
-extern "C" int sjb200_stage1_sharded_finish(sjb200_comm *m, sjb200_sharded_result *out) {
+// the minify counterpart of sjb200_stage1_shard_dev, for the second round: minify the shard again from its true incoming
+// state (carry slot 0 = that state and count 0, so the kept bytes start at d_dst[0])
+int minify_shard_from(sjb200_ctx *c, const uint8_t *d_buf, size_t len, uint32_t state_in, uint8_t *d_dst, cudaStream_t s, uint64_t *count, uint32_t *flags) {
+  if (!ensure_desc(c, len)) return SJB200_MEMALLOC;
+  CUtensorMap map;
+  bool tma = false;
+  map_for(c, kMinify, &map, d_buf, len, &tma);
+  c->h_carry[0].count = 0; c->h_carry[0].state = state_in & 7u; c->h_carry[0].ttable = 0;
+  c->h_carry[0].flags = 0; c->h_carry[0].reserved = 0;
+  if (!ok(c, cudaMemcpyAsync(c->d_carry, c->h_carry, sizeof(Carry), cudaMemcpyHostToDevice, s), "H2D carry") ||
+      !enqueue_scan(c, kMinify, &map, tma, d_buf, len, 0, tiles_of(len), true, 0x20202020u, nullptr, d_dst, 0, s) ||
+      !fetch_result(c, s) || !ok(c, cudaStreamSynchronize(s), "sync"))
+    return SJB200_UNEXPECTED_ERROR;
+  *count = c->h_carry[1].count;
+  *flags = c->h_carry[1].flags & kFlagInternal;  // as in the kernel's record: the only flag that means something to minify
+  return *flags ? SJB200_UNEXPECTED_ERROR : SJB200_SUCCESS;
+}
+
+// Complete the oldest pass in flight, which must be of `kind`: the one body of the three sharded finishes.
+int sharded_finish(sjb200_comm *m, int kind, sjb200_sharded_result *out) {
   if (!m || !out || m->tail == m->head) return SJB200_UNEXPECTED_ERROR;
   sjb200_ctx *c = m->ctx;
   DeviceGuard g(c->device);
   memset(out, 0, sizeof(*out));
-  const sjb200_comm::Step st = m->steps[m->tail % uint32_t(kXchgSteps)];
   const uint32_t slot_i = m->tail % uint32_t(kXchgSteps);
+  const sjb200_comm::Step st = m->steps[slot_i];
+  if (st.kind != kind) {  // (the pass stays in flight: the caller can still finish it with the right call)
+    c->last_error = "sharded finish: the oldest pass in flight is of another kind";
+    return SJB200_UNEXPECTED_ERROR;
+  }
   m->tail++;
   const auto t_ev = std::chrono::steady_clock::now();
   if (!ok(c, cudaEventSynchronize(m->done[slot_i]), "event sync")) return SJB200_UNEXPECTED_ERROR;  // own scan (and its stores) done
   c->xchg_evsync_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_ev).count();
   int rc = comm_collect(m, st.seq, 0);
   if (rc != SJB200_SUCCESS) return rc;
+  for (int r = 0; r < m->nranks; r++)
+    if (xchg_kind(m->h_rec[2 * r + 1]) != kind) {  // never fold one kind's counts into another's base
+      c->last_error = "sharded pass " + std::to_string(st.seq) + ": rank " + std::to_string(r) + " published a pass of another kind (every rank must enqueue the same sequence of kinds)";
+      return SJB200_UNEXPECTED_ERROR;
+    }
+  // A speculation (state 0) is wrong when the true incoming state changes what the scan keeps: for stage 1 any bit does
+  // (bit 2 decides whether a scalar starts), for minify only escape and in-string do.  validate_utf8 records carry
+  // transducer 0, so its states are all 0.
+  const uint32_t matters = (kind == kMinify) ? 3u : 7u;
   uint32_t tt[kMaxRanks], flags_all = 0;
   bool any_wrong = false;
   uint32_t state = 0, my_state = 0;
   for (int r = 0; r < m->nranks; r++) {
     tt[r] = uint32_t(m->h_rec[2 * r + 1] >> 8) & 0x3Fu;
     if (r == m->rank) my_state = state;
-    if (state != 0) any_wrong = true;
+    if ((state & matters) != 0) any_wrong = true;
     state = tt_apply(tt[r], state);
   }
   out->state_in = my_state;
@@ -1457,19 +1494,23 @@ extern "C" int sjb200_stage1_sharded_finish(sjb200_comm *m, sjb200_sharded_resul
   if (any_wrong) {
     c->xchg_second_rounds++;
     // second round: ranks whose speculation failed scan again with their true state; everybody republishes
-    if (my_state != 0) {
-      sjb200_shard_result sr;
-      rc = sjb200_stage1_shard_dev(c, st.d_buf, st.len, my_state, st.last, st.d_idx, &sr, st.stream);
+    if ((my_state & matters) != 0) {
+      if (kind == kIndex) {
+        sjb200_shard_result sr;
+        rc = sjb200_stage1_shard_dev(c, st.d_buf, st.len, my_state, st.last, st.d_idx, &sr, st.stream);
+        my_count = sr.count;
+        my_flags = sr.flags;
+      } else {
+        rc = minify_shard_from(c, st.d_buf, st.len, my_state, st.d_dst, st.stream, &my_count, &my_flags);
+      }
       if (rc != SJB200_SUCCESS) return rc;
-      my_count = sr.count;
-      my_flags = sr.flags;
       out->rescanned = 1;
     }
     ScanParams p;
     memset(&p, 0, sizeof(p));
     for (int r = 0; r < kMaxRanks; r++) p.xchg_peer[r] = m->peer[r];
     p.xchg_nranks = uint32_t(m->nranks); p.xchg_rank = uint32_t(m->rank); p.xchg_slot = window_slot(st.seq, 1); p.xchg_seq = st.seq;
-    if (!ok(c, launch_xchg_post(p, xchg_word0(st.seq, my_count), xchg_word1(st.seq, out->state_out, tt[m->rank], my_flags), st.stream), "xchg post") ||
+    if (!ok(c, launch_xchg_post(p, xchg_word0(st.seq, my_count), xchg_word1(st.seq, out->state_out, tt[m->rank], my_flags, kind), st.stream), "xchg post") ||
         !ok(c, cudaStreamSynchronize(st.stream), "sync"))
       return SJB200_UNEXPECTED_ERROR;
     c->launches++;
@@ -1488,14 +1529,50 @@ extern "C" int sjb200_stage1_sharded_finish(sjb200_comm *m, sjb200_sharded_resul
   out->total_count = total;
   out->flags = my_flags;
   out->flags_all = flags_all;
-  return ((my_flags | flags_all) & kFlagInternal) ? SJB200_UNEXPECTED_ERROR : SJB200_SUCCESS;
+  if ((my_flags | flags_all) & kFlagInternal) return SJB200_UNEXPECTED_ERROR;
+  if (kind == kMinify && ((state >> 1) & 1u)) return SJB200_UNCLOSED_STRING;  // the document ends inside a string: json_minifier.h L42-47
+  return SJB200_SUCCESS;
 }
+}  // namespace
+
+extern "C" int sjb200_stage1_sharded_enqueue(sjb200_comm *m, const uint8_t *d_shard, size_t len, int last_shard, uint32_t *d_idx, void *stream) {
+  return sharded_enqueue(m, kIndex, d_shard, len, last_shard, d_idx, nullptr, stream);
+}
+
+extern "C" int sjb200_stage1_sharded_finish(sjb200_comm *m, sjb200_sharded_result *out) { return sharded_finish(m, kIndex, out); }
 
 extern "C" int sjb200_stage1_sharded(sjb200_comm *m, const uint8_t *d_shard, size_t len, int last_shard, uint32_t *d_idx,
                                      sjb200_sharded_result *out, void *stream) {
   int rc = sjb200_stage1_sharded_enqueue(m, d_shard, len, last_shard, d_idx, stream);
   if (rc != SJB200_SUCCESS) return rc;
   return sjb200_stage1_sharded_finish(m, out);
+}
+
+extern "C" int sjb200_minify_sharded_enqueue(sjb200_comm *m, const uint8_t *d_shard, size_t len, uint8_t *d_dst, void *stream) {
+  return sharded_enqueue(m, kMinify, d_shard, len, 0, nullptr, d_dst, stream);
+}
+
+extern "C" int sjb200_minify_sharded_finish(sjb200_comm *m, sjb200_sharded_result *out) { return sharded_finish(m, kMinify, out); }
+
+extern "C" int sjb200_minify_sharded(sjb200_comm *m, const uint8_t *d_shard, size_t len, uint8_t *d_dst, sjb200_sharded_result *out, void *stream) {
+  int rc = sjb200_minify_sharded_enqueue(m, d_shard, len, d_dst, stream);
+  if (rc != SJB200_SUCCESS) return rc;
+  return sjb200_minify_sharded_finish(m, out);
+}
+
+extern "C" int sjb200_validate_utf8_sharded_enqueue(sjb200_comm *m, const uint8_t *d_shard, size_t len, void *stream) {
+  return sharded_enqueue(m, kUtf8, d_shard, len, 0, nullptr, nullptr, stream);
+}
+
+// returns 1 valid (every shard), 0 invalid, negative on a failure (CUDA, exchange timeout, kind mismatch)
+extern "C" int sjb200_validate_utf8_sharded_finish(sjb200_comm *m, sjb200_sharded_result *out) {
+  if (sharded_finish(m, kUtf8, out) != SJB200_SUCCESS) return -1;
+  return (out->flags_all & kFlagUtf8) ? 0 : 1;
+}
+
+extern "C" int sjb200_validate_utf8_sharded(sjb200_comm *m, const uint8_t *d_shard, size_t len, sjb200_sharded_result *out, void *stream) {
+  if (sjb200_validate_utf8_sharded_enqueue(m, d_shard, len, stream) != SJB200_SUCCESS) return -1;
+  return sjb200_validate_utf8_sharded_finish(m, out);
 }
 
 extern "C" uint32_t sjb200_fold_state(const uint32_t *ttables, int nshards_before) {

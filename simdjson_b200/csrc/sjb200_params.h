@@ -68,9 +68,9 @@ struct ScanParams {
   uint32_t *ticket;         // [0] next ticket, [1] CTAs finished, [2] scan4: aggregates published so far (4 words, zero between launches)
   uint32_t *park;           // scan4 with emit warps: scratch ring for parked masks, scan4_park_words(grid) words (stays in L2)
   unsigned long long *debug;  // optional [ntiles][8] timeline (globaltimer ns) for tuning; null in production
-  // multi-GPU exchange fused into the scan (scan4): the launch's last CTA stores the shard record {count, state out,
-  // transducer, flags} into EVERY rank's exchange window over NVLink (peer-mapped device memory), tagged with xchg_seq --
-  // the path's one exchange step (SURVEY.md 8e) without a collective launch.  xchg_nranks == 0: no exchange.
+  // multi-GPU exchange fused into the scan (scan4 and utf8v2): the launch's last CTA stores the shard record {count,
+  // state out, transducer, flags, kind} into EVERY rank's exchange window over NVLink (peer-mapped device memory), tagged
+  // with xchg_seq -- the path's one exchange step (SURVEY.md 8e) without a collective launch.  xchg_nranks == 0: no exchange.
   unsigned long long *xchg_peer[kMaxRanks];  // [r] = base of rank r's window: [slots][kMaxRanks][2] words
   uint32_t xchg_nranks, xchg_rank, xchg_slot, xchg_seq;
   // scan4 stage 1, several whole documents in one launch: ndocs (1..kMaxLaunchDocs) entries in device memory.  buf, len,
@@ -87,13 +87,17 @@ struct ScanParams {
 #define SJ_PARAMS_HD
 #endif
 // one shard record as two independently tagged 64-bit words (8-byte stores are single transactions):
-//   w0 = seq[30:0] << 33 | count[32:0]        w1 = seq << 32 | flags << 16 | ttable << 8 | state_out
+//   w0 = seq[30:0] << 33 | count[32:0]        w1 = seq << 32 | kind << 24 | flags << 16 | ttable << 8 | state_out
+// kind is the scan kind of the pass (kIndex 0, kMinify 1, kUtf8 2); count is structurals (kIndex), kept bytes (kMinify)
+// or 0 (kUtf8).
 SJ_PARAMS_HD inline unsigned long long xchg_word0(uint32_t seq, uint64_t count) {
   return ((unsigned long long)(seq & 0x7FFFFFFFu) << 33) | (count & 0x1FFFFFFFFull);
 }
-SJ_PARAMS_HD inline unsigned long long xchg_word1(uint32_t seq, uint32_t state, uint32_t ttable, uint32_t flags) {
-  return ((unsigned long long)seq << 32) | ((unsigned long long)(flags & 0xFFu) << 16) | ((unsigned long long)(ttable & 0x3Fu) << 8) | (state & 7u);
+SJ_PARAMS_HD inline unsigned long long xchg_word1(uint32_t seq, uint32_t state, uint32_t ttable, uint32_t flags, int kind) {
+  return ((unsigned long long)seq << 32) | ((unsigned long long)(uint32_t(kind) & 3u) << 24) | ((unsigned long long)(flags & 0xFFu) << 16) |
+         ((unsigned long long)(ttable & 0x3Fu) << 8) | (state & 7u);
 }
+SJ_PARAMS_HD inline int xchg_kind(unsigned long long w1) { return int(uint32_t(w1 >> 24) & 3u); }
 SJ_PARAMS_HD inline bool xchg_complete(unsigned long long w0, unsigned long long w1, uint32_t seq) {
   return uint32_t(w0 >> 33) == (seq & 0x7FFFFFFFu) && uint32_t(w1 >> 32) == seq;
 }

@@ -1,5 +1,6 @@
 """Multi-GPU sharding of one stage-1 scan (SURVEY.md section 8e): the host-side protocol around
-`sjb200_stage1_shard_dev`.
+`sjb200_stage1_shard_dev`, and `Comm`, the per-rank object of the sharded stage-1 / minify / validate_utf8 passes whose
+exchange is fused into the kernels.
 
 Every rank scans its byte range with a *speculated* incoming scanner state (0 = outside a string, no pending
 escape, previous byte not a scalar).  A shard's 6-bit carry transducer does not depend on the incoming state, so
@@ -97,6 +98,43 @@ class Comm:
         if rc != 0:
             return rc, None
         return self.finish()
+
+    # minify and validate_utf8 passes go through the same window; every rank must enqueue the same sequence of kinds
+    def minify_enqueue(self, d_shard, d_dst, stream=None):
+        """d_dst: uint8 device tensor of at least d_shard.numel() bytes; the shard's kept bytes are d_dst[:count]"""
+        from .implementation import _stream_ptr
+        if d_dst.numel() * d_dst.element_size() < d_shard.numel():
+            raise ValueError("d_dst needs len(shard) bytes")
+        return _lib().sjb200_minify_sharded_enqueue(self._h, d_shard.data_ptr(), d_shard.numel(), d_dst.data_ptr(), _stream_ptr(stream))
+
+    def minify_finish(self):
+        """(error_code, ShardedResult): count kept bytes at offset base of the minified document of length total_count;
+        UNCLOSED_STRING on every rank when the document ends inside a string"""
+        res = self._capi.ShardedResult()
+        rc = _lib().sjb200_minify_sharded_finish(self._h, C.byref(res))
+        return rc, res
+
+    def minify(self, d_shard, d_dst, stream=None):
+        rc = self.minify_enqueue(d_shard, d_dst, stream)
+        if rc != 0:
+            return rc, None
+        return self.minify_finish()
+
+    def validate_utf8_enqueue(self, d_shard, stream=None):
+        """cut the buffer at character boundaries (shard_cuts): then the AND of the shards' verdicts is the buffer's"""
+        from .implementation import _stream_ptr
+        return _lib().sjb200_validate_utf8_sharded_enqueue(self._h, d_shard.data_ptr(), d_shard.numel(), _stream_ptr(stream))
+
+    def validate_utf8_finish(self):
+        """(verdict, ShardedResult): 1 when the whole buffer is valid UTF-8, 0 when not, negative on a failure"""
+        res = self._capi.ShardedResult()
+        v = _lib().sjb200_validate_utf8_sharded_finish(self._h, C.byref(res))
+        return v, res
+
+    def validate_utf8(self, d_shard, stream=None):
+        if self.validate_utf8_enqueue(d_shard, stream) != 0:
+            return -1, None
+        return self.validate_utf8_finish()
 
     def close(self):
         if self._h:
