@@ -271,6 +271,83 @@ SJB200_API int sjb200_validate_utf8_sharded_enqueue(sjb200_comm *comm, const uin
 SJB200_API int sjb200_validate_utf8_sharded_finish(sjb200_comm *comm, sjb200_sharded_result *out);
 SJB200_API int sjb200_validate_utf8_sharded(sjb200_comm *comm, const uint8_t *d_shard, size_t len, sjb200_sharded_result *out, void *stream);
 
+/* stage 1 of a whitespace-separated stream (NDJSON, concatenated documents) sharded the same way, with the whole
+ * stream's finish(): `mode` is SJB200_REGULAR, SJB200_STREAMING_PARTIAL or SJB200_STREAMING_FINAL (3-6, the RS and
+ * comma-delimited streams, are rejected with UNEXPECTED_ERROR: their filters need bracket depth and separator runs carried
+ * across the cuts).  Every rank passes the same mode; last_shard = 1 on the last rank only.  In the streaming modes the
+ * last shard alone is trimmed of a partial UTF-8 character at its end (a shard that trims to nothing still takes part).
+ * Cuts at character boundaries (sjb200_shard_cut / sjb200_shard_cut_line).  A stream pass has its own kind, so a rank
+ * whose peers enqueued another kind for the same pass fails with UNEXPECTED_ERROR.
+ *
+ * finish returns, on every rank, the error code stage1(whole buffer, mode) returns, and:
+ *   n      that call's n_structural_indexes (0 on the paths where it leaves n untouched: UNCLOSED_STRING in regular
+ *          mode, UNESCAPED_CHARS, a stream that trims to nothing, an internal error);
+ *   kept   how many of this shard's structurals are among the first n: d_idx[0, kept) + bytes_before are global
+ *          structurals [shard.base, shard.base + kept);
+ *   d_idx  gathered as G = concat over ranks of d_idx[0, shard.count) + bytes_before, followed by the last rank's three
+ *          words after its count (the first two + its bytes_before), G[0, n + 3) is the whole call's index array up to
+ *          n + 3.  In streaming-final mode the words at m = n and m + 1 that the reference rewrites are rewritten by the
+ *          ranks that hold them, shard-relative (modulo 2^32);
+ *   total_bytes  the stream's length after the trim (word m of streaming-final mode);
+ *   first_starts_document  whether this shard's structural 0 starts a document (the predicate of
+ *          sjb200_document_table_dev, applied across the cut to the last structural of the previous shard that has one).
+ * Streaming modes run one more host-synchronised round than sjb200_stage1_sharded: every rank stores a small summary of
+ * its shard (walked back from its last structural to its last document start) into every window and folds them. */
+typedef struct {
+  sjb200_sharded_result shard;    /* the fold of the scan, as sjb200_stage1_sharded_finish reports it */
+  uint64_t n;
+  uint64_t kept;
+  uint64_t bytes_before;          /* byte offset of this shard in the stream */
+  uint64_t total_bytes;
+  uint32_t first_starts_document;
+  uint32_t reserved;
+} sjb200_sharded_stream_result;
+SJB200_API int sjb200_stage1_sharded_stream_enqueue(sjb200_comm *comm, const uint8_t *d_shard, size_t len, int last_shard, int mode, uint32_t *d_idx,
+                                         void *stream);
+SJB200_API int sjb200_stage1_sharded_stream_finish(sjb200_comm *comm, sjb200_sharded_stream_result *out);
+SJB200_API int sjb200_stage1_sharded_stream(sjb200_comm *comm, const uint8_t *d_shard, size_t len, int last_shard, int mode, uint32_t *d_idx,
+                                 sjb200_sharded_stream_result *out, void *stream);
+
+/* the document starts of one shard of a sharded stream pass: (local structural index, shard-relative byte) pairs of
+ * d_idx[0, kept), structural 0 counted when first_starts_document says so (both from the pass's result).  A rank's
+ * global document numbers are its table's positions plus the other ranks' ndocs before it.  Not collective.
+ * sjb200_document_table_dev is this call with first_starts_document = 1. */
+SJB200_API int sjb200_document_table_shard_dev(sjb200_ctx *ctx, const uint8_t *d_shard, const uint32_t *d_idx, uint32_t kept, int first_starts_document,
+                                    sjb200_doc_boundary *d_table, uint32_t capacity, uint32_t *ndocs_out, void *stream);
+
+/* the host fold of the streaming round, pure (no device, no comm): what every rank's finish computes from the
+ * nranks summaries.  Roles: 0 value, 1 ',' or ':', 2 '{', 3 '}', 4 '[', 5 ']'. */
+typedef struct {
+  uint64_t count;         /* in: structurals of the shard (after the second round) */
+  uint32_t len;           /* shard length after the trim */
+  uint32_t first_byte;    /* byte of structural 0 (count > 0) */
+  uint32_t last_byte;     /* byte of structural count-1 (count > 0) */
+  uint32_t start_index;   /* last document start >= 1 among the kept structurals (has_start) */
+  uint32_t start_byte;
+  int32_t net_obj;        /* '{' minus '}' from that start on, or over all kept structurals without one */
+  int32_t net_arr;        /* '[' minus ']', likewise */
+  uint32_t role_first;    /* role of the first kept structural */
+  uint32_t role_last;     /* role of the last kept structural */
+  uint32_t has_start;
+} sjb200_stream_summary;
+typedef struct {
+  uint64_t kept;
+  uint64_t bytes_before;
+  uint32_t first_starts_document;
+  uint32_t nrewrites;       /* 0..2 words of this rank's d_idx rewritten: d_idx[rewrite_pos[k]] = rewrite_val[k] */
+  uint32_t rewrite_pos[2];
+  uint32_t rewrite_val[2];
+} sjb200_stream_rank;
+typedef struct {
+  int error;
+  uint32_t n_written;       /* 0: n left untouched */
+  uint64_t n;
+  uint64_t total_bytes;
+} sjb200_stream_fold_result;
+/* final_state / flags_all as in sjb200_sharded_result.  Returns res->error. */
+SJB200_API int sjb200_stream_fold(int mode, int nranks, uint32_t final_state, uint32_t flags_all, const sjb200_stream_summary *sums,
+                       sjb200_stream_fold_result *res, sjb200_stream_rank *ranks /* nranks */);
+
 /* fold: state entering shard r given the ttables of shards 0..r-1 and the document's initial state 0 */
 SJB200_API uint32_t sjb200_fold_state(const uint32_t *ttables, int nshards_before);
 /* largest cut <= nominal such that buf[cut] is not a UTF-8 continuation byte (host pointer) */

@@ -23,6 +23,8 @@ EXPORTS = [
     "sjb200_minify_sharded", "sjb200_minify_sharded_enqueue", "sjb200_minify_sharded_finish",
     "sjb200_validate_utf8_sharded", "sjb200_validate_utf8_sharded_enqueue", "sjb200_validate_utf8_sharded_finish",
     "sjb200_tokens_dev", "sjb200_string_buf_capacity",
+    "sjb200_stage1_sharded_stream", "sjb200_stage1_sharded_stream_enqueue", "sjb200_stage1_sharded_stream_finish",
+    "sjb200_document_table_shard_dev", "sjb200_stream_fold",
 ]
 COMM_HANDLE_BYTES = 64
 
@@ -51,6 +53,26 @@ class ShardResult(C.Structure):
 class ShardedResult(C.Structure):
     _fields_ = [("count", C.c_uint64), ("base", C.c_uint64), ("total_count", C.c_uint64), ("state_in", C.c_uint32), ("state_out", C.c_uint32),
                 ("final_state", C.c_uint32), ("flags", C.c_uint32), ("flags_all", C.c_uint32), ("rescanned", C.c_uint32)]
+
+
+class ShardedStreamResult(C.Structure):
+    _fields_ = [("shard", ShardedResult), ("n", C.c_uint64), ("kept", C.c_uint64), ("bytes_before", C.c_uint64), ("total_bytes", C.c_uint64),
+                ("first_starts_document", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+class StreamSummary(C.Structure):
+    _fields_ = [("count", C.c_uint64), ("len", C.c_uint32), ("first_byte", C.c_uint32), ("last_byte", C.c_uint32), ("start_index", C.c_uint32),
+                ("start_byte", C.c_uint32), ("net_obj", C.c_int32), ("net_arr", C.c_int32), ("role_first", C.c_uint32), ("role_last", C.c_uint32),
+                ("has_start", C.c_uint32)]
+
+
+class StreamRank(C.Structure):
+    _fields_ = [("kept", C.c_uint64), ("bytes_before", C.c_uint64), ("first_starts_document", C.c_uint32), ("nrewrites", C.c_uint32),
+                ("rewrite_pos", C.c_uint32 * 2), ("rewrite_val", C.c_uint32 * 2)]
+
+
+class StreamFoldResult(C.Structure):
+    _fields_ = [("error", C.c_int), ("n_written", C.c_uint32), ("n", C.c_uint64), ("total_bytes", C.c_uint64)]
 
 
 def load():
@@ -108,6 +130,12 @@ def load():
         "sjb200_validate_utf8_sharded_finish": (C.c_int, [vp, C.POINTER(ShardedResult)]),
         "sjb200_tokens_dev": (C.c_int, [vp, vp, sz, vp, C.c_uint32, vp, vp, vp, sz, C.POINTER(TokensResult), vp]),
         "sjb200_string_buf_capacity": (sz, [sz]),
+        "sjb200_stage1_sharded_stream": (C.c_int, [vp, vp, sz, C.c_int, C.c_int, vp, C.POINTER(ShardedStreamResult), vp]),
+        "sjb200_stage1_sharded_stream_enqueue": (C.c_int, [vp, vp, sz, C.c_int, C.c_int, vp, vp]),
+        "sjb200_stage1_sharded_stream_finish": (C.c_int, [vp, C.POINTER(ShardedStreamResult)]),
+        "sjb200_document_table_shard_dev": (C.c_int, [vp, vp, vp, C.c_uint32, C.c_int, vp, C.c_uint32, u32p, vp]),
+        "sjb200_stream_fold": (C.c_int, [C.c_int, C.c_int, C.c_uint32, C.c_uint32, C.POINTER(StreamSummary), C.POINTER(StreamFoldResult),
+                                         C.POINTER(StreamRank)]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)

@@ -221,10 +221,10 @@ int grid_for(sjb200_ctx *c, int kind, uint32_t nelements) {
   return int(std::max<uint32_t>(1, std::min<uint32_t>(uint32_t(grid_cap(c, kind)), nelements)));
 }
 
-// where a sharded launch publishes its record (sjb200_comm)
+// where a sharded launch publishes its record (sjb200_comm), and the kind the record carries
 struct XchgTarget {
   unsigned long long *peer[kMaxRanks];
-  uint32_t nranks, rank, slot, seq;
+  uint32_t nranks, rank, slot, seq, kind;
 };
 
 // Option time_kernel: events around one scan launch.  time_begin records the first one and returns the second (null:
@@ -279,7 +279,7 @@ bool enqueue_scan(sjb200_ctx *c, int kind, const CUtensorMap *map, bool tma, con
   p.ticket = c->d_ticket;
   if (xchg) {  // both kernels publish the record (scan4: stage 1 and minify; utf8v2: validate_utf8)
     for (int r = 0; r < kMaxRanks; r++) p.xchg_peer[r] = xchg->peer[r];
-    p.xchg_nranks = xchg->nranks; p.xchg_rank = xchg->rank; p.xchg_slot = xchg->slot; p.xchg_seq = xchg->seq;
+    p.xchg_nranks = xchg->nranks; p.xchg_rank = xchg->rank; p.xchg_slot = xchg->slot; p.xchg_seq = xchg->seq; p.xchg_kind = xchg->kind;
   }
   p.debug = nullptr;
   if (c->opt_debug_timeline) {
@@ -833,6 +833,12 @@ extern "C" int sjb200_stage1_dev_batch(sjb200_ctx *c, sjb200_doc *docs, int ndoc
 // device-resident index array, in stream order
 extern "C" int sjb200_document_table_dev(sjb200_ctx *c, const uint8_t *d_buf, const uint32_t *d_idx, uint32_t n, sjb200_doc_boundary *d_table,
                                          uint32_t capacity, uint32_t *ndocs_out, void *stream) {
+  return sjb200_document_table_shard_dev(c, d_buf, d_idx, n, 1, d_table, capacity, ndocs_out, stream);
+}
+
+// the same for one shard of a sharded stream pass: whether structural 0 starts a document came from the pass's fold
+extern "C" int sjb200_document_table_shard_dev(sjb200_ctx *c, const uint8_t *d_buf, const uint32_t *d_idx, uint32_t n, int first_starts_document,
+                                               sjb200_doc_boundary *d_table, uint32_t capacity, uint32_t *ndocs_out, void *stream) {
   if (!c || !d_buf || !d_idx || !ndocs_out || (capacity && !d_table)) return SJB200_UNEXPECTED_ERROR;
   *ndocs_out = 0;
   if (n == 0) return SJB200_SUCCESS;
@@ -845,7 +851,8 @@ extern "C" int sjb200_document_table_dev(sjb200_ctx *c, const uint8_t *d_buf, co
     c->doc_scratch_words = need;
   }
   static_assert(sizeof(sjb200_doc_boundary) == sizeof(sjb200_doc_boundary_t), "layout");
-  if (!ok(c, launch_doc_table(d_buf, d_idx, n, c->d_doc_scratch, reinterpret_cast<sjb200_doc_boundary_t *>(d_table), capacity, c->d_ndocs, s), "doc table") ||
+  if (!ok(c, launch_doc_table(d_buf, d_idx, n, first_starts_document != 0, c->d_doc_scratch, reinterpret_cast<sjb200_doc_boundary_t *>(d_table), capacity,
+                              c->d_ndocs, s), "doc table") ||
       !ok(c, cudaMemcpyAsync(c->h_small, c->d_ndocs, sizeof(uint32_t), cudaMemcpyDeviceToHost, s), "D2H ndocs") || !ok(c, cudaStreamSynchronize(s), "sync"))
     return SJB200_UNEXPECTED_ERROR;
   c->launches += 3;
@@ -1282,35 +1289,41 @@ extern "C" int sjb200_stage1_shard_dev_enqueue(sjb200_ctx *c, const uint8_t *d_b
 struct sjb200_comm {
   sjb200_ctx *ctx = nullptr;
   int rank = 0, nranks = 1;
-  unsigned long long *window = nullptr;            // [kXchgSteps][2 rounds][kMaxRanks][2]
+  unsigned long long *window = nullptr;            // [kXchgSteps][2 rounds][kMaxRanks][2], then the summaries (sjb200_params.h)
   unsigned long long *peer[kMaxRanks] = {};        // peer[r] = rank r's window as seen from this device
   bool opened[kMaxRanks] = {};                     // mapped through cudaIpcOpenMemHandle (to be closed)
   bool connected = false;
-  unsigned long long *h_rec = nullptr;             // pinned [kMaxRanks][2]
+  unsigned long long *h_rec = nullptr;             // pinned [kMaxRanks][kSumWords]: records ([r][0..1]) or summaries
   Carry *d_result = nullptr;                       // [kXchgSteps] the launches' own result blocks
   cudaStream_t poll_stream = nullptr;
   cudaEvent_t done[kXchgSteps] = {};
-  struct Step { const uint8_t *d_buf; size_t len; uint32_t *d_idx; uint8_t *d_dst; cudaStream_t stream; uint32_t seq; int last; int kind; } steps[kXchgSteps];
+  struct Step { const uint8_t *d_buf; size_t len; uint32_t *d_idx; uint8_t *d_dst; cudaStream_t stream; uint32_t seq; int last; int kind; int mode; } steps[kXchgSteps];
   uint32_t head = 0, tail = 0;                     // passes enqueued / finished
   long poll_timeout_ms = 20000;
 };
 
 namespace {
-constexpr size_t kWindowWords = size_t(kXchgSteps) * 2 * kMaxRanks * 2;
+constexpr size_t kWindowWords = kXchgWindowWords;
 uint32_t window_slot(uint32_t seq, int round) { return (seq % uint32_t(kXchgSteps)) * 2u + uint32_t(round); }
 
-// wait (host polling, bounded) until every rank's record of (seq, round) is in the local window; records -> comm->h_rec
+// wait (host polling, bounded) until every rank's record of (seq, round) is in the local window; records -> comm->h_rec.
+// round 2: the summaries of a streaming pass (kSumWords words per rank, each tagged with seq).
 int comm_collect(sjb200_comm *m, uint32_t seq, int round) {
   sjb200_ctx *c = m->ctx;
-  const unsigned long long *src = m->window + size_t(window_slot(seq, round)) * kMaxRanks * 2;
+  const bool sums = (round == 2);
+  const unsigned long long *src = sums ? m->window + xchg_summary_at(seq, 0) : m->window + size_t(window_slot(seq, round)) * kMaxRanks * 2;
+  const size_t words = sums ? size_t(kSumWords) : 2;
   const auto t0 = std::chrono::steady_clock::now();
   for (;;) {
-    if (!ok(c, cudaMemcpyAsync(m->h_rec, src, size_t(m->nranks) * 16, cudaMemcpyDeviceToHost, m->poll_stream), "D2H window") ||
+    if (!ok(c, cudaMemcpyAsync(m->h_rec, src, size_t(m->nranks) * words * 8, cudaMemcpyDeviceToHost, m->poll_stream), "D2H window") ||
         !ok(c, cudaStreamSynchronize(m->poll_stream), "sync"))
       return SJB200_UNEXPECTED_ERROR;
     c->xchg_polls++;
     bool all = true;
-    for (int r = 0; r < m->nranks; r++) all = all && xchg_complete(m->h_rec[2 * r], m->h_rec[2 * r + 1], seq);
+    for (int r = 0; r < m->nranks; r++) {
+      if (!sums) { all = all && xchg_complete(m->h_rec[2 * r], m->h_rec[2 * r + 1], seq); continue; }
+      for (int k = 0; k < kSumWords; k++) all = all && uint32_t(m->h_rec[size_t(r) * kSumWords + k] >> 32) == seq;
+    }
     if (all) {
       c->xchg_wait_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
       return SJB200_SUCCESS;
@@ -1334,7 +1347,7 @@ extern "C" int sjb200_comm_create(sjb200_ctx *c, int rank, int nranks, sjb200_co
   bool good = dev_alloc(c, &m->window, kWindowWords, "cudaMalloc(window)") &&
               ok(c, cudaMemset(m->window, 0, kWindowWords * sizeof(unsigned long long)), "memset window") &&
               dev_alloc(c, &m->d_result, kXchgSteps, "cudaMalloc(results)") &&
-              ok(c, cudaMallocHost(&hp, kMaxRanks * 16), "cudaMallocHost") &&
+              ok(c, cudaMallocHost(&hp, kMaxRanks * kSumWords * 8), "cudaMallocHost") &&
               ok(c, cudaStreamCreateWithFlags(&m->poll_stream, cudaStreamNonBlocking), "stream");
   m->h_rec = static_cast<unsigned long long *>(hp);
   for (int i = 0; good && i < kXchgSteps; i++) good = ok(c, cudaEventCreateWithFlags(&m->done[i], cudaEventDisableTiming), "event");
@@ -1405,27 +1418,47 @@ extern "C" int sjb200_comm_connect_local(sjb200_comm *m, sjb200_comm *const *all
 namespace {
 // Enqueue one pass of `kind` (kIndex: d_idx, kMinify: d_dst, kUtf8: neither).  The launch's record lands in every rank's
 // window; m->done[slot] marks the end of the launch on `stream`.
-int sharded_enqueue(sjb200_comm *m, int kind, const uint8_t *d_shard, size_t len, int last_shard, uint32_t *d_idx, uint8_t *d_dst, void *stream) {
-  if (!m || !m->connected || !d_shard || len == 0 || len > kMaxBytes || (kind == kIndex && !d_idx) || (kind == kMinify && !d_dst))
+int sharded_enqueue(sjb200_comm *m, int kind, const uint8_t *d_shard, size_t len, int last_shard, uint32_t *d_idx, uint8_t *d_dst, void *stream,
+                    int mode = SJB200_REGULAR) {
+  const bool idx_kind = (kind == kIndex || kind == kStream);
+  if (!m || !m->connected || !d_shard || len == 0 || len > kMaxBytes || (idx_kind && !d_idx) || (kind == kMinify && !d_dst))
     return SJB200_UNEXPECTED_ERROR;
+  if (kind == kStream && (mode < SJB200_REGULAR || mode > SJB200_STREAMING_FINAL)) return SJB200_UNEXPECTED_ERROR;
   if (m->head - m->tail >= uint32_t(kXchgSteps / 2)) return SJB200_CAPACITY;  // too many passes in flight: finish some first
   sjb200_ctx *c = m->ctx;
   DeviceGuard g(c->device);
   const auto t_enq = std::chrono::steady_clock::now();
   cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
-  if (use_scan4(c, kind) && !ensure_desc(c, len)) return SJB200_MEMALLOC;
+  if (kind == kStream && last_shard && mode != SJB200_REGULAR) {  // the partial UTF-8 trim of the stream's end (json_structural_indexer.h L198-204)
+    const size_t k = std::min<size_t>(3, len);
+    if (!ok(c, cudaMemcpyAsync(c->h_small, d_shard + len - k, k, cudaMemcpyDeviceToHost, s), "D2H tail") || !ok(c, cudaStreamSynchronize(s), "sync"))
+      return SJB200_UNEXPECTED_ERROR;
+    len = trim_partial_utf8_tail(c->h_small, k, len);
+  }
+  const int scan_kind = idx_kind ? kIndex : kind;  // a stream pass scans like stage 1; only its record's kind differs
+  if (use_scan4(c, scan_kind) && len && !ensure_desc(c, len)) return SJB200_MEMALLOC;
   const uint32_t seq = m->head + 1;  // tags start at 1: a zeroed window never matches
   XchgTarget x;
   for (int r = 0; r < kMaxRanks; r++) x.peer[r] = m->peer[r];
-  x.nranks = uint32_t(m->nranks); x.rank = uint32_t(m->rank); x.slot = window_slot(seq, 0); x.seq = seq;
-  CUtensorMap map;
-  bool tma = false;
-  map_for(c, kind, &map, d_shard, len, &tma);
+  x.nranks = uint32_t(m->nranks); x.rank = uint32_t(m->rank); x.slot = window_slot(seq, 0); x.seq = seq; x.kind = uint32_t(kind);
   const uint32_t i = m->head % uint32_t(kXchgSteps);
   sjb200_comm::Step &st = m->steps[i];
-  st.d_buf = d_shard; st.len = len; st.d_idx = d_idx; st.d_dst = d_dst; st.stream = s; st.seq = seq; st.last = last_shard; st.kind = kind;
-  if (!enqueue_scan(c, kind, &map, tma, d_shard, len, 0, tiles_of(len), true, 0x20202020u, d_idx, d_dst, -1, s, 1, false, m->d_result + i, nullptr, &x) ||
-      !ok(c, cudaEventRecord(m->done[i], s), "event record"))
+  st.d_buf = d_shard; st.len = len; st.d_idx = d_idx; st.d_dst = d_dst; st.stream = s; st.seq = seq; st.last = last_shard; st.kind = kind; st.mode = mode;
+  bool good;
+  if (len == 0) {  // a last shard that trims to nothing: no scan; its record {count 0, escape passed through, no flags}
+    ScanParams p;
+    memset(&p, 0, sizeof(p));
+    for (int r = 0; r < kMaxRanks; r++) p.xchg_peer[r] = x.peer[r];
+    p.xchg_nranks = x.nranks; p.xchg_rank = x.rank; p.xchg_slot = x.slot; p.xchg_seq = seq;
+    good = ok(c, launch_xchg_post(p, xchg_word0(seq, 0), xchg_word1(seq, 0, 0x8u, 0, kind), s), "xchg post");
+    c->launches += good ? 1 : 0;
+  } else {
+    CUtensorMap map;
+    bool tma = false;
+    map_for(c, scan_kind, &map, d_shard, len, &tma);
+    good = enqueue_scan(c, scan_kind, &map, tma, d_shard, len, 0, tiles_of(len), true, 0x20202020u, d_idx, d_dst, -1, s, 1, false, m->d_result + i, nullptr, &x);
+  }
+  if (!good || !ok(c, cudaEventRecord(m->done[i], s), "event record"))
     return SJB200_UNEXPECTED_ERROR;
   m->head++;
   c->xchg_enqueue_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_enq).count();
@@ -1494,8 +1527,8 @@ int sharded_finish(sjb200_comm *m, int kind, sjb200_sharded_result *out) {
   if (any_wrong) {
     c->xchg_second_rounds++;
     // second round: ranks whose speculation failed scan again with their true state; everybody republishes
-    if ((my_state & matters) != 0) {
-      if (kind == kIndex) {
+    if ((my_state & matters) != 0 && st.len > 0) {  // (a stream's last shard that trimmed to nothing has nothing to scan)
+      if (kind != kMinify) {
         sjb200_shard_result sr;
         rc = sjb200_stage1_shard_dev(c, st.d_buf, st.len, my_state, st.last, st.d_idx, &sr, st.stream);
         my_count = sr.count;
@@ -1533,7 +1566,194 @@ int sharded_finish(sjb200_comm *m, int kind, sjb200_sharded_result *out) {
   if (kind == kMinify && ((state >> 1) & 1u)) return SJB200_UNCLOSED_STRING;  // the document ends inside a string: json_minifier.h L42-47
   return SJB200_SUCCESS;
 }
+
+// Complete the oldest pass in flight, a stream pass: the scan's fold (sharded_finish), then the summary round and the
+// host fold of the whole stream's finish() (sjb200_stream_fold), then this rank's sentinels and rewrites.
+int sharded_stream_finish(sjb200_comm *m, sjb200_sharded_stream_result *out) {
+  if (!m || !out || m->tail == m->head) return SJB200_UNEXPECTED_ERROR;
+  memset(out, 0, sizeof(*out));
+  const sjb200_comm::Step st = m->steps[m->tail % uint32_t(kXchgSteps)];
+  int rc = sharded_finish(m, kStream, &out->shard);
+  if (rc != SJB200_SUCCESS) return rc;  // (an internal error is seen by every rank alike: nobody runs the summary round)
+  sjb200_ctx *c = m->ctx;
+  DeviceGuard g(c->device);
+  // h_rec holds every rank's last record: the counts after the second round
+  uint64_t counts[kMaxRanks];
+  int holder = -1;  // the rank that holds the stream's last structural
+  for (int r = 0; r < m->nranks; r++) {
+    counts[r] = xchg_count(m->h_rec[2 * r]);
+    if (counts[r]) holder = r;
+  }
+  const bool unclosed = (out->shard.final_state >> 1) & 1u;
+  const uint64_t my_count = counts[m->rank];
+  const uint64_t kept = my_count - ((st.mode != SJB200_REGULAR && unclosed && holder == m->rank) ? 1 : 0);
+  ScanParams x;
+  memset(&x, 0, sizeof(x));
+  for (int r = 0; r < kMaxRanks; r++) x.xchg_peer[r] = m->peer[r];
+  x.xchg_nranks = uint32_t(m->nranks); x.xchg_rank = uint32_t(m->rank); x.xchg_seq = st.seq;
+  if (!ok(c, launch_stream_summary(st.d_buf, st.d_idx, uint32_t(my_count), uint32_t(kept), uint32_t(st.len), st.mode != SJB200_REGULAR, x, m->poll_stream),
+          "stream summary"))
+    return SJB200_UNEXPECTED_ERROR;
+  c->launches++;
+  rc = comm_collect(m, st.seq, 2);
+  if (rc != SJB200_SUCCESS) return rc;
+  sjb200_stream_summary sums[kMaxRanks];
+  for (int r = 0; r < m->nranks; r++) {
+    const unsigned long long *w = m->h_rec + size_t(r) * kSumWords;
+    sjb200_stream_summary &s = sums[r];
+    s.count = counts[r];
+    s.len = uint32_t(w[0]); s.first_byte = uint32_t(w[1]); s.last_byte = uint32_t(w[2]);
+    s.start_index = uint32_t(w[3]); s.start_byte = uint32_t(w[4]);
+    s.net_obj = int32_t(uint32_t(w[5])); s.net_arr = int32_t(uint32_t(w[6]));
+    s.role_first = uint32_t(w[7]) & 7u; s.role_last = (uint32_t(w[7]) >> 3) & 7u; s.has_start = (uint32_t(w[7]) >> 6) & 1u;
+  }
+  sjb200_stream_fold_result res;
+  sjb200_stream_rank ranks[kMaxRanks];
+  const int err = sjb200_stream_fold(st.mode, m->nranks, out->shard.final_state, out->shard.flags_all, sums, &res, ranks);
+  const sjb200_stream_rank &me = ranks[m->rank];
+  out->n = res.n;
+  out->kept = me.kept;
+  out->bytes_before = me.bytes_before;
+  out->total_bytes = res.total_bytes;
+  out->first_starts_document = me.first_starts_document;
+  // the stream's sentinels (json_structural_indexer.h L284-286) go behind the last rank's count, then the final fix-up
+  const bool sentinels = res.n_written && st.last;
+  if (sentinels || me.nrewrites) {
+    if ((sentinels && !ok(c, launch_write_sentinels(st.d_idx, uint32_t(my_count), uint32_t(st.len), uint32_t(st.len), 0, m->poll_stream), "sentinels")) ||
+        (me.nrewrites && !ok(c, launch_store_words(st.d_idx, me.nrewrites, me.rewrite_pos[0], me.rewrite_val[0], me.rewrite_pos[1], me.rewrite_val[1],
+                                                  m->poll_stream), "rewrite")) ||
+        !ok(c, cudaStreamSynchronize(m->poll_stream), "sync"))
+      return SJB200_UNEXPECTED_ERROR;
+    c->launches += (sentinels ? 1 : 0) + (me.nrewrites ? 1 : 0);
+  }
+  return err;
+}
 }  // namespace
+
+extern "C" int sjb200_stage1_sharded_stream_enqueue(sjb200_comm *m, const uint8_t *d_shard, size_t len, int last_shard, int mode, uint32_t *d_idx,
+                                                    void *stream) {
+  return sharded_enqueue(m, kStream, d_shard, len, last_shard, d_idx, nullptr, stream, mode);
+}
+
+extern "C" int sjb200_stage1_sharded_stream_finish(sjb200_comm *m, sjb200_sharded_stream_result *out) { return sharded_stream_finish(m, out); }
+
+extern "C" int sjb200_stage1_sharded_stream(sjb200_comm *m, const uint8_t *d_shard, size_t len, int last_shard, int mode, uint32_t *d_idx,
+                                            sjb200_sharded_stream_result *out, void *stream) {
+  int rc = sjb200_stage1_sharded_stream_enqueue(m, d_shard, len, last_shard, mode, d_idx, stream);
+  if (rc != SJB200_SUCCESS) return rc;
+  return sjb200_stage1_sharded_stream_finish(m, out);
+}
+
+namespace {
+enum : uint32_t { kRoleValue = 0, kRoleSep, kRoleOpenObj, kRoleCloseObj, kRoleOpenArr, kRoleCloseArr };  // as in sjb200_docs.cu
+bool starts_document(uint32_t cur, uint32_t before) {  // find_next_document_index.h L60-88
+  if (cur == kRoleSep || cur == kRoleCloseObj || cur == kRoleCloseArr) return false;
+  return !(before == kRoleOpenObj || before == kRoleOpenArr || before == kRoleSep);
+}
+}  // namespace
+
+// The fold of the summaries into the whole stream's finish() (json_structural_indexer.h L249-343, L395-396).  T = all
+// structurals, n0 = T less the stream's last one when it ends inside a string (streaming modes).  The last document start
+// g of [0, n0) is the last internal start of the last shard that has one, unless the first structural of a later shard
+// starts a document across its cut; the brackets from g on are that shard's nets after its start plus the later shards'
+// nets.  Then m = n0 when they balance, else g (0 without any start), as find_next_document_index.
+extern "C" int sjb200_stream_fold(int mode, int nranks, uint32_t final_state, uint32_t flags_all, const sjb200_stream_summary *sums,
+                                  sjb200_stream_fold_result *res, sjb200_stream_rank *ranks) {
+  if (!res || !ranks || !sums || nranks < 1 || nranks > kMaxRanks || mode < SJB200_REGULAR || mode > SJB200_STREAMING_FINAL) return SJB200_UNEXPECTED_ERROR;
+  memset(res, 0, sizeof(*res));
+  memset(ranks, 0, sizeof(*ranks) * size_t(nranks));
+  uint64_t base[kMaxRanks], off = 0, T = 0;
+  int holder = -1;
+  for (int r = 0; r < nranks; r++) {
+    ranks[r].bytes_before = off;
+    off += sums[r].len;
+    base[r] = T;
+    T += sums[r].count;
+    if (sums[r].count) holder = r;
+  }
+  const uint64_t L = off;
+  res->total_bytes = L;
+  const bool streaming = mode != SJB200_REGULAR, unclosed = (final_state >> 1) & 1u;
+  auto done = [&](int err) {
+    res->error = err;
+    for (int r = 0; r < nranks && res->n_written; r++) {
+      const uint64_t k = res->n > base[r] ? res->n - base[r] : 0;
+      ranks[r].kept = std::min<uint64_t>(k, sums[r].count);
+    }
+    for (int r = 0, prev = -1; r < nranks; r++) {  // prev: the last earlier shard with kept structurals
+      if (ranks[r].kept == 0) continue;
+      ranks[r].first_starts_document = (prev < 0) ? 1u : uint32_t(starts_document(sums[r].role_first, sums[prev].role_last));
+      prev = r;
+    }
+    return err;
+  };
+  if (flags_all & kFlagInternal) return done(SJB200_UNEXPECTED_ERROR);
+  if (streaming && L == 0) return done(SJB200_UTF8_ERROR);           // L198-204: nothing left after the trim
+  if (!streaming && unclosed) return done(SJB200_UNCLOSED_STRING);   // L255-259
+  if (flags_all & kFlagCtl) return done(SJB200_UNESCAPED_CHARS);    // L261-263
+  res->n_written = 1;
+  res->n = T;
+  if (T == 0) return done(SJB200_EMPTY);                             // L289-291
+  const bool utf8 = (flags_all & kFlagUtf8) != 0;
+  if (!streaming) return done(utf8 ? SJB200_UTF8_ERROR : SJB200_SUCCESS);
+  const uint64_t n0 = T - (unclosed ? 1 : 0);
+  if (mode == SJB200_STREAMING_PARTIAL && unclosed && n0 == 0) { res->n = 0; return done(SJB200_CAPACITY); }  // L298-302
+  // the last document start g < n0 and the bracket balance of [g, n0); gv = global byte of structural g
+  uint64_t g = 0, gv = 0;
+  bool found = false;
+  int64_t nobj = 0, narr = 0;
+  for (int r = nranks - 1; r >= 0 && !found; r--) {
+    const uint64_t kp = sums[r].count - ((unclosed && r == holder) ? 1 : 0);
+    if (kp == 0) continue;
+    nobj += sums[r].net_obj;
+    narr += sums[r].net_arr;
+    if (sums[r].has_start) {
+      found = true; g = base[r] + sums[r].start_index; gv = ranks[r].bytes_before + sums[r].start_byte;
+    } else if (base[r] > 0) {
+      int q = r - 1;
+      while (q >= 0 && sums[q].count == 0) q--;
+      if (q >= 0 && starts_document(sums[r].role_first, sums[q].role_last)) { found = true; g = base[r]; gv = ranks[r].bytes_before + sums[r].first_byte; }
+    }
+  }
+  if (!found && n0 > 0) {  // the start is structural 0
+    int r0 = 0;
+    while (sums[r0].count == 0) r0++;
+    gv = ranks[r0].bytes_before + sums[r0].first_byte;
+  }
+  const uint64_t m = (n0 == 0) ? 0 : ((nobj == 0 && narr == 0) ? n0 : g);
+  if (mode == SJB200_STREAMING_PARTIAL) {  // L303-317
+    if (m == 0) {
+      const bool idx0_zero = sums[0].count > 0 && sums[0].first_byte == 0;
+      if (idx0_zero) { res->n = n0; return done(SJB200_CAPACITY); }
+      res->n = 0;
+      return done(SJB200_EMPTY);
+    }
+    res->n = m;
+    return done(utf8 ? SJB200_UTF8_ERROR : SJB200_SUCCESS);
+  }
+  // streaming final, L329-343: word m + 1 = old word m, word m = L; the ranks that hold them store them shard-relative
+  uint64_t old_m;
+  if (m >= T) old_m = L;                                                            // a sentinel
+  else if (m == T - 1 && unclosed) old_m = ranks[holder].bytes_before + sums[holder].last_byte;  // the dropped quote
+  else old_m = gv;                                                                  // a document start
+  const uint64_t pos[2] = {m, m + 1}, val[2] = {L, old_m};
+  for (int k = 0; k < 2; k++) {
+    int r = nranks - 1;
+    uint64_t local = sums[r].count + (pos[k] - T);
+    if (pos[k] < T) {
+      r = 0;
+      while (!(pos[k] >= base[r] && pos[k] < base[r] + sums[r].count)) r++;
+      local = pos[k] - base[r];
+    }
+    sjb200_stream_rank &w = ranks[r];
+    w.rewrite_pos[w.nrewrites] = uint32_t(local);
+    w.rewrite_val[w.nrewrites] = uint32_t(val[k] - w.bytes_before);
+    w.nrewrites++;
+  }
+  res->n = m;
+  if (m == 0) return done(SJB200_EMPTY);
+  return done(utf8 ? SJB200_UTF8_ERROR : SJB200_SUCCESS);
+}
 
 extern "C" int sjb200_stage1_sharded_enqueue(sjb200_comm *m, const uint8_t *d_shard, size_t len, int last_shard, uint32_t *d_idx, void *stream) {
   return sharded_enqueue(m, kIndex, d_shard, len, last_shard, d_idx, nullptr, stream);

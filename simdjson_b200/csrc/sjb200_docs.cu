@@ -69,14 +69,16 @@ __device__ int block_max(int v, int *sh) {
   return s;
 }
 
-// complete_document_count (find_next_document_index.h L39-98) on a device-resident array: walk back from the end in
-// windows of kFinishThreads structurals until a window holds a document start; one CTA.  Returns (to every thread) the
-// number of structurals that belong to complete documents.
-__device__ uint32_t complete_count(const uint8_t *buf, const uint32_t *idx, uint32_t n, int *sh) {
-  if (n == 0) return 0;
+// The backward walk of find_next_document_index (find_next_document_index.h L39-98) on a device-resident array: from
+// structural n-1 back in windows of kFinishThreads structurals until a window holds a document start i >= 1; one CTA.
+// Every thread gets *start = that i (-1 when there is none) and the object / array bracket nets of structurals
+// [*start, n), or of [0, n) when there is no start.
+__device__ void last_document_start(const uint8_t *buf, const uint32_t *idx, uint32_t n, int *sh, int *start, int *nobj_out, int *narr_out) {
   int nobj = 0, narr = 0;  // opens minus closes over the structurals after the current window
   uint32_t hi = n;
+  *start = -1;
   for (;;) {
+    if (hi == 0) break;
     const uint32_t lo = hi > uint32_t(kFinishThreads) ? hi - uint32_t(kFinishThreads) : 0u;
     const uint32_t i = lo + threadIdx.x;
     const bool in = i < hi;
@@ -85,18 +87,30 @@ __device__ uint32_t complete_count(const uint8_t *buf, const uint32_t *idx, uint
       r = role_of(buf[idx[i]]);
       if (i > 0) before = role_of(buf[idx[i - 1]]);
     }
-    const bool start = in && i >= 1 && starts_document(r, before);
-    const int last = block_max(start ? int(i) : -1, sh);
-    if (last >= 0) {  // the last document starts at `last`: complete iff its brackets balance
+    const bool is_start = in && i >= 1 && starts_document(r, before);
+    const int last = block_max(is_start ? int(i) : -1, sh);
+    if (last >= 0) {  // the last document starts at `last`
       const bool tail = in && int(i) >= last;
-      const int o = block_sum(tail ? net_obj(r) : 0, sh), a = block_sum(tail ? net_arr(r) : 0, sh);
-      return (nobj + o == 0 && narr + a == 0) ? n : uint32_t(last);
+      nobj += block_sum(tail ? net_obj(r) : 0, sh);
+      narr += block_sum(tail ? net_arr(r) : 0, sh);
+      *start = last;
+      break;
     }
     nobj += block_sum(in ? net_obj(r) : 0, sh);
     narr += block_sum(in ? net_arr(r) : 0, sh);
-    if (lo == 0) return (nobj == 0 && narr == 0) ? n : 0u;  // one document from the very first structural on
     hi = lo;
   }
+  *nobj_out = nobj;
+  *narr_out = narr;
+}
+
+// complete_document_count: the number of structurals that belong to complete documents (to every thread).  The last
+// document is complete iff its brackets balance; without an internal start it is one document from structural 0 on.
+__device__ uint32_t complete_count(const uint8_t *buf, const uint32_t *idx, uint32_t n, int *sh) {
+  if (n == 0) return 0;
+  int start, nobj, narr;
+  last_document_start(buf, idx, n, sh, &start, &nobj, &narr);
+  return (nobj == 0 && narr == 0) ? n : (start >= 0 ? uint32_t(start) : 0u);
 }
 
 // the streaming branches of finish() (modes 1 and 2) behind a device-resident scan
@@ -145,20 +159,56 @@ __global__ void __launch_bounds__(kFinishThreads) stream_finish_kernel(const uin
   }
 }
 
+// The summary of one shard for the extra round of a sharded streaming pass: walk back from the shard's last kept
+// structural to its last internal document start (index >= 1), then store the kSumWords-word summary (sjb200_params.h)
+// into every rank's window.  kept = the shard's structurals, less the stream's last one when the stream ends inside a
+// string and this shard holds it; walk = 0 (regular mode) skips the walk.
+__global__ void __launch_bounds__(kFinishThreads) stream_summary_kernel(const uint8_t *buf, const uint32_t *idx, uint32_t count, uint32_t kept, uint32_t len,
+                                                                       int walk, ScanParams x) {
+  __shared__ int sh[kFinishThreads / 32];
+  int start = -1, nobj = 0, narr = 0;
+  if (walk && kept > 0) last_document_start(buf, idx, kept, sh, &start, &nobj, &narr);
+  const uint32_t r = threadIdx.x;
+  if (r < x.xchg_nranks) {
+    uint32_t w[kSumWords];
+    w[0] = len;
+    w[1] = count ? idx[0] : 0u;
+    w[2] = count ? idx[count - 1] : 0u;
+    w[3] = start >= 0 ? uint32_t(start) : 0u;
+    w[4] = start >= 0 ? idx[start] : 0u;
+    w[5] = uint32_t(nobj);
+    w[6] = uint32_t(narr);
+    w[7] = (kept ? role_of(buf[idx[0]]) | (role_of(buf[idx[kept - 1]]) << 3) : 0u) | (start >= 0 ? 1u << 6 : 0u);
+    unsigned long long *rec = x.xchg_peer[r] + xchg_summary_at(x.xchg_seq, x.xchg_rank);
+    for (int k = 0; k < kSumWords; k++) {
+      const unsigned long long v = (static_cast<unsigned long long>(x.xchg_seq) << 32) | w[k];
+      asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(rec + k), "l"(v) : "memory");
+    }
+  }
+}
+
+// a sharded streaming pass's rewrite of the words it holds (at most two)
+__global__ void store_words_kernel(uint32_t *idx, uint32_t nw, uint32_t p0, uint32_t v0, uint32_t p1, uint32_t v1) {
+  if (nw > 0) idx[p0] = v0;
+  if (nw > 1) idx[p1] = v1;
+}
+
 // ---------------------------------------------------------------------------------------------- document table
 constexpr int kTabThreads = 256, kTabPerThread = 8, kTabTile = kTabThreads * kTabPerThread;
 
-__device__ __forceinline__ bool doc_start_at(const uint8_t *buf, const uint32_t *idx, uint32_t i) {
-  if (i == 0) return true;
+// first_starts: whether structural 0 starts a document (always, for a whole stream; for a shard, by the predicate
+// applied across the cut)
+__device__ __forceinline__ bool doc_start_at(const uint8_t *buf, const uint32_t *idx, uint32_t i, bool first_starts) {
+  if (i == 0) return first_starts;
   return starts_document(role_of(buf[idx[i]]), role_of(buf[idx[i - 1]]));
 }
-__global__ void __launch_bounds__(kTabThreads) doc_count_kernel(const uint8_t *buf, const uint32_t *idx, uint32_t n, uint32_t *tile_count) {
+__global__ void __launch_bounds__(kTabThreads) doc_count_kernel(const uint8_t *buf, const uint32_t *idx, uint32_t n, bool first_starts, uint32_t *tile_count) {
   __shared__ uint32_t sh[kTabThreads / 32];
   const uint32_t base = blockIdx.x * kTabTile;
   uint32_t c = 0;
   for (int k = 0; k < kTabPerThread; k++) {
     const uint32_t i = base + k * kTabThreads + threadIdx.x;
-    if (i < n && doc_start_at(buf, idx, i)) c++;
+    if (i < n && doc_start_at(buf, idx, i, first_starts)) c++;
   }
   for (int d = 16; d > 0; d >>= 1) c += __shfl_down_sync(0xFFFFFFFFu, c, d);
   if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = c;
@@ -202,8 +252,8 @@ __global__ void __launch_bounds__(1024) doc_scan_kernel(uint32_t *tile_count, ui
   }
   if (threadIdx.x == 0) *ndocs = carry;
 }
-__global__ void __launch_bounds__(kTabThreads) doc_write_kernel(const uint8_t *buf, const uint32_t *idx, uint32_t n, const uint32_t *tile_offset,
-                                                               sjb200_doc_boundary_t *table, uint32_t capacity) {
+__global__ void __launch_bounds__(kTabThreads) doc_write_kernel(const uint8_t *buf, const uint32_t *idx, uint32_t n, bool first_starts,
+                                                               const uint32_t *tile_offset, sjb200_doc_boundary_t *table, uint32_t capacity) {
   __shared__ uint32_t warp_base[kTabThreads / 32];
   __shared__ uint32_t running;
   if (threadIdx.x == 0) running = tile_offset[blockIdx.x];
@@ -211,7 +261,7 @@ __global__ void __launch_bounds__(kTabThreads) doc_write_kernel(const uint8_t *b
   const uint32_t base = blockIdx.x * kTabTile;
   for (int k = 0; k < kTabPerThread; k++) {  // consecutive threads take consecutive structurals: table order = stream order
     const uint32_t i = base + k * kTabThreads + threadIdx.x;
-    const bool f = i < n && doc_start_at(buf, idx, i);
+    const bool f = i < n && doc_start_at(buf, idx, i, first_starts);
     const uint32_t bal = __ballot_sync(0xFFFFFFFFu, f);
     const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     if (lane == 0) warp_base[warp] = __popc(bal);
@@ -483,13 +533,24 @@ cudaError_t launch_stream_finish(const uint8_t *buf, uint32_t *idx, const Carry 
 
 size_t doc_table_scratch_words(uint32_t n) { return size_t((n + kTabTile - 1) / kTabTile) + 1; }
 
-cudaError_t launch_doc_table(const uint8_t *buf, const uint32_t *idx, uint32_t n, uint32_t *scratch, sjb200_doc_boundary_t *table, uint32_t capacity,
-                             uint32_t *ndocs_dev, cudaStream_t stream) {
+cudaError_t launch_doc_table(const uint8_t *buf, const uint32_t *idx, uint32_t n, bool first_starts, uint32_t *scratch, sjb200_doc_boundary_t *table,
+                             uint32_t capacity, uint32_t *ndocs_dev, cudaStream_t stream) {
   const uint32_t ntiles = (n + kTabTile - 1) / kTabTile;
   if (ntiles == 0) return cudaMemsetAsync(ndocs_dev, 0, sizeof(uint32_t), stream);
-  doc_count_kernel<<<ntiles, kTabThreads, 0, stream>>>(buf, idx, n, scratch);
+  doc_count_kernel<<<ntiles, kTabThreads, 0, stream>>>(buf, idx, n, first_starts, scratch);
   doc_scan_kernel<<<1, 1024, 0, stream>>>(scratch, ntiles, ndocs_dev);
-  doc_write_kernel<<<ntiles, kTabThreads, 0, stream>>>(buf, idx, n, scratch, table, capacity);
+  doc_write_kernel<<<ntiles, kTabThreads, 0, stream>>>(buf, idx, n, first_starts, scratch, table, capacity);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_stream_summary(const uint8_t *buf, const uint32_t *idx, uint32_t count, uint32_t kept, uint32_t len, int walk, const ScanParams &x,
+                                  cudaStream_t stream) {
+  stream_summary_kernel<<<1, kFinishThreads, 0, stream>>>(buf, idx, count, kept, len, walk, x);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_store_words(uint32_t *idx, uint32_t nw, uint32_t p0, uint32_t v0, uint32_t p1, uint32_t v1, cudaStream_t stream) {
+  store_words_kernel<<<1, 1, 0, stream>>>(idx, nw, p0, v0, p1, v1);
   return cudaGetLastError();
 }
 

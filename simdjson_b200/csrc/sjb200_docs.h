@@ -29,9 +29,15 @@ cudaError_t launch_stream_finish(const uint8_t *buf, uint32_t *idx, const Carry 
 size_t filter_scratch_words(uint32_t n);
 cudaError_t launch_stream_filter(const uint8_t *buf, uint32_t len, uint32_t *idx, uint32_t n, int mode, uint32_t flags, uint32_t *scratch, StreamFinish *out_dev,
                                  StreamFinish *out_host, cudaStream_t stream);
-// table of document starts of a whitespace-separated stream; scratch: doc_table_scratch_words(n) uint32 words
+// table of document starts of a whitespace-separated stream; scratch: doc_table_scratch_words(n) uint32 words.
+// first_starts: whether structural 0 starts a document (true for a whole stream; for a shard, as the stream fold said)
 size_t doc_table_scratch_words(uint32_t n);
-cudaError_t launch_doc_table(const uint8_t *buf, const uint32_t *idx, uint32_t n, uint32_t *scratch, sjb200_doc_boundary_t *table, uint32_t capacity,
-                             uint32_t *ndocs_dev, cudaStream_t stream);
+cudaError_t launch_doc_table(const uint8_t *buf, const uint32_t *idx, uint32_t n, bool first_starts, uint32_t *scratch, sjb200_doc_boundary_t *table,
+                             uint32_t capacity, uint32_t *ndocs_dev, cudaStream_t stream);
+// sharded streaming passes: the shard's summary into every rank's window (fields xchg_* of x; layout in sjb200_params.h)
+cudaError_t launch_stream_summary(const uint8_t *buf, const uint32_t *idx, uint32_t count, uint32_t kept, uint32_t len, int walk, const ScanParams &x,
+                                  cudaStream_t stream);
+// ... and the rewrite of the (at most two) words of the final fix-up this rank holds
+cudaError_t launch_store_words(uint32_t *idx, uint32_t nw, uint32_t p0, uint32_t v0, uint32_t p1, uint32_t v1, cudaStream_t stream);
 
 }  // namespace sjb200

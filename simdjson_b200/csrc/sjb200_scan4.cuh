@@ -1267,7 +1267,7 @@ SJ_DEV void scan4_body(const sj_tensor_map *tmap, const ScanParams &p, uint8_t *
         // (minify validates nothing: of its flags only an internal error means something -- a shard cut inside a UTF-8
         // character or a control character in a string is not an error of minify)
         const unsigned long long w0 = xchg_word0(p.xchg_seq, co->count),
-                                 w1 = xchg_word1(p.xchg_seq, co->state, co->ttable, kMode == 2 ? (fl & uint32_t(kFlagInternal)) : fl, kMode == 2 ? kMinify : kIndex);
+                                 w1 = xchg_word1(p.xchg_seq, co->state, co->ttable, kMode == 2 ? (fl & uint32_t(kFlagInternal)) : fl, kMode == 2 ? kMinify : int(p.xchg_kind));
         for (uint32_t r = 0; r < p.xchg_nranks; r++) {
           unsigned long long *rec = p.xchg_peer[r] + (size_t(p.xchg_slot) * kMaxRanks + p.xchg_rank) * 2;
           sj_st_sys_u64(rec, w0);

@@ -23,6 +23,23 @@ def fold_states(ttables):
     return [int(L.sjb200_fold_state(arr, r)) for r in range(len(ttables))]
 
 
+def fold_stream(mode, final_state, flags_all, summaries):
+    """sjb200_stream_fold: summaries = one dict per shard with the fields of sjb200_stream_summary.  Returns
+    (error, n_written, n, total_bytes, [per rank dict(kept, bytes_before, first_starts_document, rewrites=[(pos, val)])])"""
+    from . import capi
+    k = len(summaries)
+    sums = (capi.StreamSummary * k)()
+    for s, d in zip(sums, summaries):
+        for name, _ in capi.StreamSummary._fields_:
+            setattr(s, name, int(d.get(name, 0)))
+    res = capi.StreamFoldResult()
+    ranks = (capi.StreamRank * k)()
+    _lib().sjb200_stream_fold(int(mode), k, int(final_state), int(flags_all), sums, C.byref(res), ranks)
+    out = [{"kept": int(r.kept), "bytes_before": int(r.bytes_before), "first_starts_document": int(r.first_starts_document),
+            "rewrites": [(int(r.rewrite_pos[j]), int(r.rewrite_val[j])) for j in range(r.nrewrites)]} for r in ranks]
+    return int(res.error), int(res.n_written), int(res.n), int(res.total_bytes), out
+
+
 def shard_cuts(buf, nshards):
     """cut a host buffer into nshards byte ranges at UTF-8 character boundaries"""
     L = _lib()
@@ -135,6 +152,41 @@ class Comm:
         if self.validate_utf8_enqueue(d_shard, stream) != 0:
             return -1, None
         return self.validate_utf8_finish()
+
+    # stage 1 of a whitespace-separated stream with the whole stream's finish() (modes REGULAR, STREAMING_PARTIAL,
+    # STREAMING_FINAL); its passes share the window with the other kinds
+    def stream_enqueue(self, d_shard, d_idx, last_shard, mode, stream=None):
+        from .implementation import _stream_ptr
+        return _lib().sjb200_stage1_sharded_stream_enqueue(self._h, d_shard.data_ptr(), d_shard.numel(), int(last_shard), int(mode), d_idx.data_ptr(),
+                                                           _stream_ptr(stream))
+
+    def stream_finish(self):
+        """(error_code, ShardedStreamResult): the error code and n of stage1(whole stream, mode) on every rank; this
+        shard's kept structurals d_idx[:kept] + bytes_before, total_bytes, first_starts_document"""
+        res = self._capi.ShardedStreamResult()
+        rc = _lib().sjb200_stage1_sharded_stream_finish(self._h, C.byref(res))
+        return rc, res
+
+    def scan_stream(self, d_shard, d_idx, last_shard, mode, stream=None):
+        rc = self.stream_enqueue(d_shard, d_idx, last_shard, mode, stream)
+        if rc != 0:
+            return rc, None
+        return self.stream_finish()
+
+    def document_table(self, d_shard, d_idx, result, stream=None):
+        """the document starts among this shard's kept structurals (result: a ShardedStreamResult): (local structural
+        index, shard-relative byte) pairs as an int64 [ndocs, 2] CPU array.  Not collective."""
+        import torch
+
+        from .implementation import _stream_ptr
+        kept = int(result.kept)
+        table = torch.empty(max(kept, 1) * 2, dtype=torch.int32, device=d_idx.device)
+        nd = C.c_uint32(0)
+        rc = _lib().sjb200_document_table_shard_dev(self.parser._ctx, d_shard.data_ptr(), d_idx.data_ptr(), kept, int(result.first_starts_document),
+                                                    table.data_ptr(), max(kept, 1), C.byref(nd), _stream_ptr(stream))
+        if rc != 0:
+            raise RuntimeError(f"sjb200_document_table_shard_dev failed ({rc}): " + self.parser.last_cuda_error())
+        return table[: 2 * nd.value].cpu().numpy().view(np.uint32).astype(np.int64).reshape(-1, 2)
 
     def close(self):
         if self._h:
