@@ -86,17 +86,23 @@ SJB200_API int sjb200_device(const sjb200_ctx *ctx);
 SJB200_API const char *sjb200_last_cuda_error(const sjb200_ctx *ctx);
 /* tuning knobs, mostly for tests and bench: "use_tma" (0/1), "grid" (CTAs, 0 = auto), "chunk_bytes", "copy_threads",
  * "ew_min_bytes" (stage-1 launches of at least this size use the emit-warp build of the kernel; 0 = never),
- * "time_kernel" (0/1: record CUDA events around the scan kernel on its launch stream); none changes results */
+ * "time_kernel" (0/1: record CUDA events around the scan kernel on its launch stream), "pdl" (0/1, default 1: the
+ * scan launches of one sjb200_stage1_dev_batch call after the first may start while the previous one still runs),
+ * "launch_stamps" (0/1: sjb200_get_launch_stamps); none changes results */
 SJB200_API int sjb200_set_option(sjb200_ctx *ctx, const char *key, long value);
 /* "kernel_ms" (last scan kernel, needs time_kernel=1), "kernel_ms_mean" (the scan kernels since the previous query),
  * both per document: a launch that scans several documents (sjb200_stage1_dev_batch) counts its duration divided by
- * their number; "launches" (kernels launched by this context so far),
+ * their number, and a sjb200_stage1_dev_batch call counts the span from its first scan launch to the end of its last
+ * one (launches may overlap), divided by its documents; "launches" (kernels launched by this context so far),
  * "ew_launches" (of which on the emit-warp build),
  * "grid_index", "sm_count"; negative when unavailable */
 SJB200_API double sjb200_get_stat(sjb200_ctx *ctx, const char *key);
 
 /* tuning aid (option "debug_timeline"=1): per-tile phase timestamps of the last launch, 8 x uint64 per tile */
 SJB200_API long sjb200_get_debug_timeline(sjb200_ctx *ctx, unsigned long long *out, size_t max_tiles);
+/* tuning aid (option "launch_stamps"=1): for every scan launch of the last sjb200_stage1_dev_batch call, the globaltimer
+ * (ns) at its first CTA's entry and at its last CTA's exit (0 for a group of one document); returns the launches copied */
+SJB200_API long sjb200_get_launch_stamps(sjb200_ctx *ctx, unsigned long long *out, size_t max_launches);
 
 /* page-lock / unlock caller-owned host memory (e.g. the parser's `new uint32_t[]` index array, whose deleter the
  * reference fixes: internal/dom_parser_implementation.h L175) so copies to it run at full PCIe speed; best effort */

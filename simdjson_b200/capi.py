@@ -13,6 +13,7 @@ LIB_PATH = os.environ.get("SJB200_LIB") or os.path.join(_HERE, "libsjb200.so")  
 EXPORTS = [
     "sjb200_create", "sjb200_destroy", "sjb200_set_capacity", "sjb200_capacity", "sjb200_index_words", "sjb200_device",
     "sjb200_last_cuda_error", "sjb200_set_option", "sjb200_get_stat", "sjb200_pin_host_memory", "sjb200_unpin_host_memory", "sjb200_get_debug_timeline",
+    "sjb200_get_launch_stamps",
     "sjb200_stage1", "sjb200_minify", "sjb200_validate_utf8",
     "sjb200_stage1_dev", "sjb200_minify_dev", "sjb200_validate_utf8_dev", "sjb200_stage1_dev_batch",
     "sjb200_document_table_dev", "sjb200_stage1_dev_enqueue", "sjb200_stage1_dev_finish", "sjb200_minify_dev_enqueue", "sjb200_minify_dev_finish",
@@ -93,6 +94,7 @@ def load():
         "sjb200_set_option": (C.c_int, [vp, C.c_char_p, C.c_long]),
         "sjb200_get_stat": (C.c_double, [vp, C.c_char_p]),
         "sjb200_get_debug_timeline": (C.c_long, [vp, vp, sz]),
+        "sjb200_get_launch_stamps": (C.c_long, [vp, vp, sz]),
         "sjb200_pin_host_memory": (C.c_int, [vp, vp, sz]),
         "sjb200_unpin_host_memory": (C.c_int, [vp, vp]),
         "sjb200_stage1": (C.c_int, [vp, vp, sz, C.c_int, vp, u32p]),

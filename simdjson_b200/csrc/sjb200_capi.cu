@@ -30,6 +30,14 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap *, CUtensorMapDataType, cuuint32
                                     CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
 constexpr int kCarrySlots = 1024;
+constexpr int kTmapCacheEntries = 64;
+
+struct TmapCacheEntry {
+  const uint8_t *base = nullptr;
+  uint64_t rows = 0;
+  int box_rows = 0;
+  CUtensorMap map;
+};
 constexpr size_t kMaxBytes = 0xFFFFFFFFull;  // SIMDJSON_MAXSIZE_BYTES (include/simdjson/base.h L23)
 
 struct PendingCall {
@@ -59,10 +67,13 @@ struct sjb200_ctx {
   uint32_t *d_idx = nullptr;  size_t d_idx_words = 0;
   uint8_t *d_out = nullptr;   size_t d_out_bytes = 0;
   Carry *d_carry = nullptr;   // [kCarrySlots] one per chunk boundary of the chunked host pipeline
-  uint32_t *d_flags = nullptr;  // [0] the launch's flags, [1 + slot] the flags of the document whose result goes to carry slot `slot`
-  uint32_t *d_ticket = nullptr;
-  unsigned long long *d_count_desc = nullptr;
+  // [0] the launch's flags, [1 + slot] the flags of the document whose result goes to carry slot `slot`, [1 + kCarrySlots]
+  // the flags of a launch of parity 1 (launch_flags)
+  uint32_t *d_flags = nullptr;
+  uint32_t *d_ticket = nullptr;  // [parity][4]
+  unsigned long long *d_count_desc = nullptr;  // [parity][desc_tiles]
   size_t desc_tiles = 0;
+  unsigned long long *d_stamps = nullptr; size_t stamps_cap = 0; size_t stamps_used = 0;  // option launch_stamps: [launch][2]
   StreamFinish *d_sfin = nullptr;  // [kCarrySlots] results of the device-side streaming epilogue
   uint32_t *d_doc_scratch = nullptr; size_t doc_scratch_words = 0; uint32_t *d_ndocs = nullptr;
   void *d_tok_scratch = nullptr; size_t tok_scratch_bytes = 0; TokenTotals *d_tok_tot = nullptr;  // stage-2-lite (sjb200_tape.cu)
@@ -88,10 +99,12 @@ struct sjb200_ctx {
   // batch round into pinned memory, copied group by group ahead of the launches
   uint8_t *h_doctab = nullptr; uint8_t *d_doctab = nullptr; size_t doctab_bytes = 0;
   long opt_debug_timeline = 0;
+  long opt_pdl = 1, opt_launch_stamps = 0;
   unsigned long long *d_debug = nullptr; size_t debug_tiles = 0; uint32_t debug_last_tiles = 0;
   unsigned long long launches = 0;               // kernels of ours launched by this context
   unsigned long long ew_launches = 0;            // ... of which stage-1 launches on the emit-warp build
   PFN_encodeTiled encode = nullptr;
+  TmapCacheEntry tmap_cache[kTmapCacheEntries];  // make_tensor_map
   // host-pointer pipeline: ring of page-locked staging slots filled by copy threads (sjb200_hostpipe.h)
   uint8_t *h_ring = nullptr; size_t ring_slot_bytes = 0; int ring_slots = 0;
   std::vector<cudaEvent_t> ring_events;
@@ -155,15 +168,15 @@ void free_sized(sjb200_ctx *c) {
 }
 
 // look-back descriptors: sized for the capacity, zeroed once (epoch tags make them reusable).  `need` descriptors: one per
-// tile is more than one per element.
+// tile is more than one per element.  Two sets, one per launch parity (launch_desc).
 bool ensure_desc_n(sjb200_ctx *c, size_t need) {
   need = std::max<size_t>(need, 1);
   if (need <= c->desc_tiles) return true;
   cudaFree(c->d_count_desc); c->d_count_desc = nullptr;
   c->desc_tiles = 0;
   const size_t n = std::max(need, size_t(tiles_of(c->capacity)) + 1);
-  if (!dev_alloc(c, &c->d_count_desc, n, "cudaMalloc(count_desc)")) return false;
-  if (!ok(c, cudaMemsetAsync(c->d_count_desc, 0, n * sizeof(unsigned long long), c->stream), "memset desc")) return false;
+  if (!dev_alloc(c, &c->d_count_desc, 2 * n, "cudaMalloc(count_desc)")) return false;
+  if (!ok(c, cudaMemsetAsync(c->d_count_desc, 0, 2 * n * sizeof(unsigned long long), c->stream), "memset desc")) return false;
   if (!ok(c, cudaStreamSynchronize(c->stream), "sync")) return false;
   c->desc_tiles = n;
   c->epoch = 0;
@@ -172,16 +185,26 @@ bool ensure_desc_n(sjb200_ctx *c, size_t need) {
 bool ensure_desc(sjb200_ctx *c, size_t len) { return ensure_desc_n(c, tiles_of(len)); }
 
 // The wipe at the wrap of the 18-bit tag is ordered on the LAUNCH stream (a context is used on one stream at a time,
-// see sjb200.h): kernels queued earlier on it finish before the wipe, the next launch starts after it.
-bool next_epoch(sjb200_ctx *c, cudaStream_t launch_stream, uint32_t *epoch) {
+// see sjb200.h): kernels queued earlier on it finish before the wipe, the next launch starts after it.  *wiped: the
+// wipe was queued (it then sits between the previous launch and the next one).
+bool next_epoch(sjb200_ctx *c, cudaStream_t launch_stream, uint32_t *epoch, bool *wiped = nullptr) {
   c->epoch++;
+  if (wiped) *wiped = false;
   if (c->epoch >= (1u << 18)) {
-    if (!ok(c, cudaMemsetAsync(c->d_count_desc, 0, c->desc_tiles * sizeof(unsigned long long), launch_stream), "memset desc")) return false;
+    if (!ok(c, cudaMemsetAsync(c->d_count_desc, 0, 2 * c->desc_tiles * sizeof(unsigned long long), launch_stream), "memset desc")) return false;
     c->epoch = 1;
+    if (wiped) *wiped = true;
   }
   *epoch = c->epoch;
   return true;
 }
+
+// The scratch a stage-1 launch re-arms for the next one -- ticket block, launch flags word, look-back descriptors -- in
+// two sets.  Two consecutive scan launches of a batch call may run at once (programmatic dependent launch): they use
+// alternate sets, and a launch starts only after the one two before it has completed.  Every other launch uses set 0.
+uint32_t *launch_ticket(sjb200_ctx *c, int parity) { return c->d_ticket + 4 * parity; }
+uint32_t *launch_flags(sjb200_ctx *c, int parity) { return parity ? c->d_flags + 1 + kCarrySlots : c->d_flags; }
+unsigned long long *launch_desc(sjb200_ctx *c, int parity) { return c->d_count_desc + size_t(parity) * c->desc_tiles; }
 
 bool make_tensor_map(sjb200_ctx *c, CUtensorMap *map, const uint8_t *d_buf, size_t len, bool *usable, int box_rows = kScan4BoxRows) {
   memset(map, 0, sizeof(*map));
@@ -189,6 +212,15 @@ bool make_tensor_map(sjb200_ctx *c, CUtensorMap *map, const uint8_t *d_buf, size
   const uint64_t rows = len / 128;
   if (!c->opt_use_tma || c->encode == nullptr || rows == 0) return true;
   if ((reinterpret_cast<uintptr_t>(d_buf) & 15u) != 0) return true;  // TMA needs a 16-byte aligned base
+  // A map is a function of (base, rows, box) alone; re-encoding it costs ~1 us of host time per document, which a batch
+  // call of many documents pays before its first launch.  Recently encoded maps are kept in a small direct-mapped cache.
+  const uintptr_t key = reinterpret_cast<uintptr_t>(d_buf);
+  TmapCacheEntry &ce = c->tmap_cache[((key >> 4) ^ (key >> 12) ^ rows ^ uint64_t(box_rows)) % kTmapCacheEntries];
+  if (ce.base == d_buf && ce.rows == rows && ce.box_rows == box_rows) {
+    *map = ce.map;
+    *usable = true;
+    return true;
+  }
   cuuint64_t dims[2] = {128, rows};
   cuuint64_t strides[1] = {128};
   cuuint32_t box[2] = {128, (cuuint32_t)box_rows};
@@ -200,6 +232,10 @@ bool make_tensor_map(sjb200_ctx *c, CUtensorMap *map, const uint8_t *d_buf, size
     c->last_error = "cuTensorMapEncodeTiled failed (" + std::to_string(int(r)) + "); using plain loads";
     return true;
   }
+  ce.base = d_buf;
+  ce.rows = rows;
+  ce.box_rows = box_rows;
+  ce.map = *map;
   *usable = true;
   return true;
 }
@@ -254,7 +290,7 @@ void time_end(sjb200_ctx *c, cudaStream_t stream, cudaEvent_t e1, bool launched,
 bool enqueue_scan(sjb200_ctx *c, int kind, const CUtensorMap *map, bool tma, const uint8_t *d_buf, size_t len, uint32_t tile_begin,
                   uint32_t ntiles, bool has_last_tile, uint32_t prev_word, uint32_t *d_idx, uint8_t *d_dst, int carry_in_slot,
                   cudaStream_t stream, int carry_out_slot = -1, bool write_sentinels = false, Carry *external_out = nullptr,
-                  Carry *host_out = nullptr, const XchgTarget *xchg = nullptr) {
+                  Carry *host_out = nullptr, const XchgTarget *xchg = nullptr, bool timed = true) {
   // carry_in_slot < 0: the launch starts a document (zero state, zero count)
   if (carry_out_slot < 0) carry_out_slot = (carry_in_slot < 0) ? 1 : (carry_in_slot ^ 1);
   ScanParams p;
@@ -290,7 +326,7 @@ bool enqueue_scan(sjb200_ctx *c, int kind, const CUtensorMap *map, bool tma, con
     }
     if (c->d_debug) { cudaMemsetAsync(c->d_debug, 0, size_t(rows) * 64, stream); p.debug = c->d_debug; c->debug_last_tiles = rows; }
   }
-  cudaEvent_t e1 = time_begin(c, stream);
+  cudaEvent_t e1 = timed ? time_begin(c, stream) : nullptr;
   bool launched;
   if (use_scan4(c, kind)) {
     const uint32_t tpe = uint32_t(scan4_tiles_per_element());
@@ -367,10 +403,10 @@ extern "C" int sjb200_create(int device, size_t capacity, sjb200_ctx **out) {
   bool good = ok(c, cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking), "stream") &&
               ok(c, cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking), "stream") &&
               ok(c, cudaStreamCreateWithFlags(&c->out_stream, cudaStreamNonBlocking), "stream") &&
-              dev_alloc(c, &c->d_carry, kCarrySlots, "cudaMalloc(carry)") && dev_alloc(c, &c->d_flags, 1 + kCarrySlots, "cudaMalloc(flags)") &&
-              dev_alloc(c, &c->d_ticket, 4, "cudaMalloc(ticket)") &&
-              ok(c, cudaMemset(c->d_ticket, 0, 4 * sizeof(uint32_t)), "memset ticket") &&
-              ok(c, cudaMemset(c->d_flags, 0, (1 + kCarrySlots) * sizeof(uint32_t)), "memset flags");
+              dev_alloc(c, &c->d_carry, kCarrySlots, "cudaMalloc(carry)") && dev_alloc(c, &c->d_flags, 2 + kCarrySlots, "cudaMalloc(flags)") &&
+              dev_alloc(c, &c->d_ticket, 8, "cudaMalloc(ticket)") &&
+              ok(c, cudaMemset(c->d_ticket, 0, 8 * sizeof(uint32_t)), "memset ticket") &&
+              ok(c, cudaMemset(c->d_flags, 0, (2 + kCarrySlots) * sizeof(uint32_t)), "memset flags");
   void *hp = nullptr;
   good = good && ok(c, cudaMallocHost(&hp, kCarrySlots * sizeof(Carry)), "cudaMallocHost");
   c->h_carry = static_cast<Carry *>(hp);
@@ -414,7 +450,7 @@ extern "C" void sjb200_destroy(sjb200_ctx *c) {
   DeviceGuard g(c->device);
   if (c->stream) cudaStreamSynchronize(c->stream);
   free_sized(c);
-  cudaFree(c->d_carry); cudaFree(c->d_flags); cudaFree(c->d_ticket); cudaFree(c->d_sfin); cudaFree(c->d_doc_scratch); cudaFree(c->d_ndocs); cudaFree(c->d_tok_scratch); cudaFree(c->d_tok_tot); cudaFree(c->d_tails); cudaFree(c->d_tail_ptrs); cudaFree(c->d_debug); cudaFree(c->d_park); cudaFree(c->d_doctab);
+  cudaFree(c->d_carry); cudaFree(c->d_flags); cudaFree(c->d_ticket); cudaFree(c->d_sfin); cudaFree(c->d_doc_scratch); cudaFree(c->d_ndocs); cudaFree(c->d_tok_scratch); cudaFree(c->d_tok_tot); cudaFree(c->d_tails); cudaFree(c->d_tail_ptrs); cudaFree(c->d_debug); cudaFree(c->d_park); cudaFree(c->d_doctab); cudaFree(c->d_stamps);
   if (c->h_doctab) cudaFreeHost(c->h_doctab);
   if (c->h_carry) cudaFreeHost(c->h_carry);
   if (c->h_flags) cudaFreeHost(c->h_flags);
@@ -456,6 +492,14 @@ extern "C" long sjb200_get_debug_timeline(sjb200_ctx *c, unsigned long long *out
   const size_t n = std::min<size_t>(max_tiles, c->debug_last_tiles);
   cudaDeviceSynchronize();
   if (cudaMemcpy(out, c->d_debug, n * 64, cudaMemcpyDeviceToHost) != cudaSuccess) { (void)cudaGetLastError(); return 0; }
+  return long(n);
+}
+
+extern "C" long sjb200_get_launch_stamps(sjb200_ctx *c, unsigned long long *out, size_t max_launches) {
+  if (!c || !c->d_stamps || !out) return 0;
+  DeviceGuard g(c->device);
+  const size_t n = std::min(max_launches, c->stamps_used);
+  if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpy(out, c->d_stamps, n * 16, cudaMemcpyDeviceToHost) != cudaSuccess) { (void)cudaGetLastError(); return 0; }
   return long(n);
 }
 
@@ -515,6 +559,8 @@ extern "C" int sjb200_set_option(sjb200_ctx *c, const char *key, long value) {
   else if (!strcmp(key, "tok_stage")) c->opt_tok_stage = value ? 1 : 0;
   else if (!strcmp(key, "time_kernel")) c->opt_time_kernel = value;
   else if (!strcmp(key, "debug_timeline")) c->opt_debug_timeline = value;
+  else if (!strcmp(key, "pdl")) c->opt_pdl = value ? 1 : 0;
+  else if (!strcmp(key, "launch_stamps")) c->opt_launch_stamps = value ? 1 : 0;
   else if (!strcmp(key, "chunk_bytes")) c->opt_chunk_bytes = std::max<long>(2 * kTileBytes, (value / (2 * kTileBytes)) * (2 * kTileBytes));
   else if (!strcmp(key, "force_grid")) c->opt_force_grid = value;
   else if (!strcmp(key, "ew_min_bytes")) c->opt_ew_min_bytes = value;
@@ -555,14 +601,16 @@ bool stage1_prepare(sjb200_ctx *c, PendingCall &pc, const uint8_t *d_buf, size_t
 }
 
 // whitespace-separated streams: the rest of finish() (find_next_document_index, the final fix-up) runs on the device
-// right behind the scan -- no host round trip between the two (sjb200_docs.cu)
-void stage1_stream_epilogue(sjb200_ctx *c, PendingCall &pc) {
+// right behind the scan -- no host round trip between the two (sjb200_docs.cu).  Returns whether it queued anything.
+bool stage1_stream_epilogue(sjb200_ctx *c, PendingCall &pc) {
   if (pc.mode == SJB200_STREAMING_PARTIAL || pc.mode == SJB200_STREAMING_FINAL) {
     c->launches++;
     const int slot = pc.carry_slot;
     if (!ok(c, launch_stream_finish(pc.d_buf, pc.d_idx, c->d_carry + slot, uint32_t(pc.len), pc.mode, c->d_sfin + slot, c->h_sfin + slot, pc.stream), "stream finish"))
       pc.early_error = SJB200_UNEXPECTED_ERROR;
+    return true;
   }
+  return false;
 }
 
 // enqueue one device-resident stage-1 scan; its {count,state,flags} come back in h_carry[slot]
@@ -664,7 +712,11 @@ size_t out_bytes(const PendingCall &pc) { return 4 * (pc.len + 3); }  // at most
 // Enqueue the scans of the prepared calls (those without an early error), consecutive documents grouped into one
 // multi-document launch each.  A group ends before a document that reads or writes memory an earlier document of the
 // group writes, or writes memory it reads: the launches then keep the order of a one-by-one loop.  The tables of all
-// groups are encoded into pinned memory first; each is copied ahead of its launch, nothing waits for the device.
+// groups are encoded into pinned memory and go to the device in one copy before the first launch, so that nothing sits
+// on the stream between two scan launches: a multi-document launch right behind another one starts while that one
+// still runs (programmatic dependent launch, option pdl) and waits for it only before an access that could conflict
+// (sjb200_scan4.cuh, wait_previous_launch).  Nothing waits for the device.  With time_kernel, one event pair spans all
+// launches of the call (overlapping launches have no duration of their own).
 int enqueue_doc_groups(sjb200_ctx *c, std::vector<PendingCall> &calls, cudaStream_t s) {
   constexpr uint64_t kMaxGroupElems = 1u << 20;  // 64 GiB of input; 8 MiB of look-back descriptors
   const uint32_t tpe = uint32_t(scan4_tiles_per_element());
@@ -704,21 +756,11 @@ int enqueue_doc_groups(sjb200_ctx *c, std::vector<PendingCall> &calls, cudaStrea
     c->doctab_bytes = off.back();
   }
   static_assert(sizeof(DocEntry) == 64 && sizeof(CUtensorMap) == 128, "table layout");
+  std::vector<uint32_t> g_elems_of(groups.size(), 0), g_tiles_of(groups.size(), 0);
   for (size_t g = 0; g < groups.size(); g++) {
     const std::vector<int> &G = groups[g];
-    if (G.size() == 1) {
-      PendingCall &pc = calls[size_t(G[0])];
-      CUtensorMap map;
-      bool tma = false;
-      map_for(c, kIndex, &map, pc.d_buf, pc.len, &tma);
-      if (!enqueue_scan(c, kIndex, &map, tma, pc.d_buf, pc.len, 0, tiles_of(pc.len), true, 0x20202020u, pc.d_idx, nullptr, -1, s, pc.carry_slot, true,
-                        nullptr, c->h_carry + pc.carry_slot))
-        pc.early_error = SJB200_UNEXPECTED_ERROR;
-      else
-        stage1_stream_epilogue(c, pc);
-      continue;
-    }
     const size_t n = G.size();
+    if (n == 1) continue;
     DocEntry *he = reinterpret_cast<DocEntry *>(c->h_doctab + off[g]);
     const size_t maps_at = off[g] + ((n * sizeof(DocEntry) + 127) & ~size_t(127));
     CUtensorMap *hm = reinterpret_cast<CUtensorMap *>(c->h_doctab + maps_at);
@@ -742,33 +784,84 @@ int enqueue_doc_groups(sjb200_ctx *c, std::vector<PendingCall> &calls, cudaStrea
       elems += e.nelem;
       tiles += tiles_of(pc.len);
     }
+    g_elems_of[g] = elems;
+    g_tiles_of[g] = tiles;
+  }
+  if (off.back() > 0 && !ok(c, cudaMemcpyAsync(c->d_doctab, c->h_doctab, off.back(), cudaMemcpyHostToDevice, s), "H2D doc tables")) return SJB200_UNEXPECTED_ERROR;
+  // early[g]: no input byte of group g lies in an index array of group g - 1, so its scan may read before that one is done
+  // (the groups' carries and flags words are distinct slots of the context, no input of a caller)
+  std::vector<char> early(groups.size(), 1);
+  for (size_t g = 1; g < groups.size(); g++)
+    for (int i : groups[g])
+      for (int j : groups[g - 1])
+        if (ranges_overlap(calls[size_t(i)].d_buf, calls[size_t(i)].len, calls[size_t(j)].d_idx, out_bytes(calls[size_t(j)]))) early[g] = 0;
+  unsigned long long *stamps = nullptr;
+  c->stamps_used = 0;
+  if (c->opt_launch_stamps) {
+    if (c->stamps_cap < groups.size()) {
+      cudaFree(c->d_stamps); c->d_stamps = nullptr; c->stamps_cap = 0;
+      if (!dev_alloc(c, &c->d_stamps, 2 * groups.size(), "cudaMalloc(stamps)")) return SJB200_MEMALLOC;
+      c->stamps_cap = groups.size();
+    }
+    if (!ok(c, cudaMemsetAsync(c->d_stamps, 0, 16 * groups.size(), s), "memset stamps")) return SJB200_UNEXPECTED_ERROR;
+    stamps = c->d_stamps;
+    c->stamps_used = groups.size();
+  }
+  cudaEvent_t e1 = time_begin(c, s);
+  uint32_t timed_docs = 0;
+  bool chained = false;  // the last operation on s is this call's previous multi-document scan launch
+  int parity = 0;
+  for (size_t g = 0; g < groups.size(); g++) {
+    const std::vector<int> &G = groups[g];
+    if (G.size() == 1) {
+      PendingCall &pc = calls[size_t(G[0])];
+      CUtensorMap map;
+      bool tma = false;
+      map_for(c, kIndex, &map, pc.d_buf, pc.len, &tma);
+      if (!enqueue_scan(c, kIndex, &map, tma, pc.d_buf, pc.len, 0, tiles_of(pc.len), true, 0x20202020u, pc.d_idx, nullptr, -1, s, pc.carry_slot, true,
+                        nullptr, c->h_carry + pc.carry_slot, nullptr, false)) {
+        pc.early_error = SJB200_UNEXPECTED_ERROR;
+      } else {
+        timed_docs++;
+        stage1_stream_epilogue(c, pc);
+      }
+      chained = false;
+      continue;
+    }
+    const size_t n = G.size();
     ScanParams p;
     memset(&p, 0, sizeof(p));
     p.prev_word = 0x20202020u;
     p.check_eof = 1;
     p.write_sentinels = 1;
-    p.ntiles = tiles;
-    p.flags = c->d_flags;
-    p.count_desc = c->d_count_desc;
-    p.ticket = c->d_ticket;
+    p.ntiles = g_tiles_of[g];
     p.docs = reinterpret_cast<const DocEntry *>(c->d_doctab + off[g]);
     p.ndocs = uint32_t(n);
-    bool good = next_epoch(c, s, &p.epoch) &&
-                ok(c, cudaMemcpyAsync(c->d_doctab + off[g], c->h_doctab + off[g], off[g + 1] - off[g], cudaMemcpyHostToDevice, s), "H2D doc table");
+    p.early_input = early[g] ? 1u : 0u;
+    p.stamps = stamps ? stamps + 2 * g : nullptr;
+    bool wiped = false;
+    bool good = next_epoch(c, s, &p.epoch, &wiped);
+    const bool pdl = good && chained && !wiped && c->opt_pdl;
+    parity = pdl ? parity ^ 1 : 0;
+    p.flags = launch_flags(c, parity);
+    p.count_desc = launch_desc(c, parity);
+    p.ticket = launch_ticket(c, parity);
     if (good) {
       CUtensorMap unused;
       memset(&unused, 0, sizeof(unused));
-      cudaEvent_t e1 = time_begin(c, s);
-      good = ok(c, launch_scan4(&unused, p, grid_for(c, kIndex, elems), 0, s), "launch scan4 (documents)");
-      time_end(c, s, e1, good, uint32_t(n));
+      good = ok(c, launch_scan4(&unused, p, grid_for(c, kIndex, g_elems_of[g]), 0, s, pdl), "launch scan4 (documents)");
       c->launches += good ? 1 : 0;
+      timed_docs += good ? uint32_t(n) : 0u;
     }
+    bool epilogue = false;
     for (size_t k = 0; k < n; k++) {
       PendingCall &pc = calls[size_t(G[k])];
-      if (good) stage1_stream_epilogue(c, pc);
+      if (good) epilogue = stage1_stream_epilogue(c, pc) || epilogue;
       else pc.early_error = SJB200_UNEXPECTED_ERROR;
     }
+    chained = good && !epilogue;
   }
+  time_end(c, s, e1, timed_docs > 0, timed_docs);
   return SJB200_SUCCESS;
 }
 }  // namespace

@@ -73,7 +73,7 @@ __global__ void xchg_post_kernel(ScanParams p, unsigned long long w0, unsigned l
 }
 
 // ------------------------------------------------------------------ launchers
-cudaError_t launch_scan4(const CUtensorMap *tmap, const ScanParams &p, int grid, int mode, cudaStream_t stream) {
+cudaError_t launch_scan4(const CUtensorMap *tmap, const ScanParams &p, int grid, int mode, cudaStream_t stream, bool pdl) {
   static bool configured[64] = {};
   int dev = 0;
   cudaGetDevice(&dev);
@@ -82,6 +82,19 @@ cudaError_t launch_scan4(const CUtensorMap *tmap, const ScanParams &p, int grid,
     if (e == cudaSuccess) e = cudaFuncSetAttribute(scan4_minify_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, scan4::kSmemBytes4);
     if (e != cudaSuccess) return e;
     if (dev >= 0 && dev < 64) configured[dev] = true;
+  }
+  if (pdl && mode == 0) {
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr.val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(unsigned(grid));
+    cfg.blockDim = dim3(unsigned(scan4::kThreads4));
+    cfg.dynamicSmemBytes = size_t(scan4::kSmemBytes4);
+    cfg.stream = stream;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+    return cudaLaunchKernelEx(&cfg, scan4_kernel, *tmap, p);
   }
   if (mode == 2) scan4_minify_kernel<<<grid, scan4::kThreads4, scan4::kSmemBytes4, stream>>>(*tmap, p);
   else scan4_kernel<<<grid, scan4::kThreads4, scan4::kSmemBytes4, stream>>>(*tmap, p);

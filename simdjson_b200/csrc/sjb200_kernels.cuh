@@ -10,9 +10,11 @@
 namespace sjb200 {
 
 // launchers (defined in sjb200_kernels.cu)
-// scan4: the stage-1 indexer of sjb200_scan4.cuh (4 KiB blocks; its tensor map has a 32-row box)
+// scan4: the stage-1 indexer of sjb200_scan4.cuh (4 KiB blocks; its tensor map has a 32-row box).  pdl (stage 1 only):
+// programmatic dependent launch -- the kernel may start while the previous operation on the stream, a scan4 stage-1
+// launch, is still running (ScanParams::early_input)
 cudaError_t launch_scan4(const CUtensorMap *tmap, const ScanParams &p, int grid, int mode /*0 stage 1, 2 minify*/,
-                         cudaStream_t stream);
+                         cudaStream_t stream, bool pdl = false);
 size_t scan4_park_words(int grid);   // uint32 words of ScanParams::park for a launch of `grid` CTAs (emit-warp builds)
 int scan4_tiles_per_element();      // 32 KiB tiles of the launch parameter block per scan4 element
 int scan4_parks_in_global();         // 1: every scan4 launch needs ScanParams::park (emit warps read the parked masks from an L2-resident ring)

@@ -81,6 +81,13 @@ struct ScanParams {
   // ndocs = 0: one document described by the scalar fields above.
   const DocEntry *docs;
   uint32_t ndocs;
+  // Programmatic dependent launch (scan4): the launch may start while the previous launch on the stream still runs, and
+  // waits for it (griddepcontrol.wait) before its first access that could conflict -- its first index store, carry,
+  // sentinel or per-document flags hand-over.  early_input = 1: no input byte lies in memory the previous launch writes,
+  // so the input may be read before that wait; 0: everything waits at the top.  ticket, flags and count_desc must not be
+  // the previous launch's (the host alternates two sets).
+  uint32_t early_input;
+  unsigned long long *stamps;  // optional [2]: globaltimer at the first CTA's entry and at the last CTA's exit (tuning)
 };
 
 #if defined(__CUDACC__)

@@ -161,6 +161,28 @@ SJ_DEV Eff compose(const Eff &o, const Eff &n) {
   return r;
 }
 
+// ------------------------------------------------------------------------------------------------ the previous launch
+// A launch may start while the previous one on the stream is still running (programmatic dependent launch, ScanParams::
+// early_input).  Every access that could conflict with it comes after this call, and so does the CTA's trigger: the
+// launch after this one then starts only once the one before this one has completed, so the ticket block, flags word
+// and descriptors of the launch parity it reuses are free again.
+SJ_DEV void wait_previous_launch() {
+  sj_griddep_wait();
+  sj_griddep_launch_dependents();
+}
+
+// A bounded wait's budget: true once a wait has polled kSpinLimit4 times after the previous launch has completed.  A
+// launch that started early may wait on elements that its CTAs scan only after their wait for the previous launch, so
+// the first exhausted budget waits for that launch and starts again.
+SJ_DEV bool spun_out(uint32_t *spins) {
+  const uint32_t s = ++*spins;
+  if ((s & 0x7FFFFFFFu) <= kSpinLimit4) return false;
+  if (s & 0x80000000u) return true;
+  sj_griddep_wait();
+  *spins = 0x80000000u;
+  return false;
+}
+
 // A waiting warp must not spin at full speed: mbarrier.try_wait returns at once, and a busy loop takes issue slots
 // from the warps that do the work.  `ns` = back-off between polls.
 #ifndef SJB200_SCAN4_POLL_SCALE
@@ -169,7 +191,7 @@ SJ_DEV Eff compose(const Eff &o, const Eff &n) {
 SJ_DEV bool wait_bar(sj_mbar_t *bar, uint32_t parity, const ScanParams &p, unsigned ns) {
   uint32_t spins = 0;
   while (!sj_mbar_try_wait(bar, parity)) {
-    if (++spins > kSpinLimit4) {
+    if (spun_out(&spins)) {
       sj_atomic_or(p.flags, kFlagInternal);
       return false;
     }
@@ -888,6 +910,7 @@ SJ_DEV void scan_role(Smem *S, const sj_tensor_map *tmap, const ScanParams &p, c
     SJ_TRACE4(6);
     SJ_TRACE4(7);
     if (!kEmitW && j >= uint32_t(kLag)) {  // pipelined: the chain warp has had kLag scans' time to resolve this one
+      if (j == uint32_t(kLag)) wait_previous_launch();  // the first emit: the previous launch may write the same index array
       wait_bar(&S->resolved[ne % kNS], (ne / kNS) & 1u, p, 64);
       SJ_TRACE4(8);
       if (!SJB200_SCAN4_TRACE && p.debug != nullptr && warp == 0 && lane == 0) p.debug[uint64_t(S->ticket[ne % kNS]) * 8 + 2] = sj_globaltimer();
@@ -913,6 +936,7 @@ SJ_DEV void scan_role(Smem *S, const sj_tensor_map *tmap, const ScanParams &p, c
     // nothing left to scan: help with what is left to emit (both ring slots are free: slot 0 is the staging area)
     emit_role<kMode>(S, tmap, p, cin, lane, S->ring[warp][0], &S->full[warp][0], full_phase & 1u);
   } else {
+    if (ne < j) wait_previous_launch();  // (the CTA scanned kLag elements or fewer: nothing emitted yet)
     while (ne < j) {
       wait_bar(&S->resolved[ne % kNS], (ne / kNS) & 1u, p, 64);
       if (kMin) {
@@ -938,6 +962,7 @@ SJ_DEV void emit_role(Smem *S, const sj_tensor_map *tmap, const ScanParams &p, c
   const uint64_t out_base = cin.count;
   const uint64_t launch_start = uint64_t(p.tile_begin) * kTileBytes;
   uint32_t *stg = reinterpret_cast<uint32_t *>(stage);
+  wait_previous_launch();  // before the first emit
   for (;;) {
     uint32_t q = 0;
     if (lane == 0) q = sj_atomic_add(&S->emit_next, 1u);
@@ -949,7 +974,7 @@ SJ_DEV void emit_role(Smem *S, const sj_tensor_map *tmap, const ScanParams &p, c
       if (sj_mbar_try_wait(&S->resolved[e % kNS], (e / kNS) & 1u)) break;
       const uint32_t done = sj_ld_acquire_u32(&S->scan_done);
       if (done != 0xFFFFFFFFu && e >= done) return;
-      if (++spins > kSpinLimit4) {
+      if (spun_out(&spins)) {
         sj_atomic_or(p.flags, kFlagInternal);
         return;
       }
@@ -1036,7 +1061,7 @@ SJ_DEV void look_back(const ScanParams &p, uint32_t t, unsigned lane, uint32_t *
         needed = (1u << nk) - 1u;
       }
       if (!sj_any((pend & needed) != 0)) break;
-      if (++spins > kSpinLimit4) {  // never expected: report, and finish with what there is
+      if (spun_out(&spins)) {  // never expected: report, and finish with what there is
         sj_atomic_or(p.flags, kFlagInternal);
         break;
       }
@@ -1156,7 +1181,10 @@ SJ_DEV void chain_role(Smem *S, const ScanParams &p, const Carry &cin, unsigned 
     sj_syncwarp();
     if (lane == 0) sj_mbar_arrive(&S->resolved[ns]);
     if (!SJB200_SCAN4_TRACE && p.debug != nullptr && lane == 0) p.debug[uint64_t(t) * 8 + 4] = sj_globaltimer();
-    if (t == D.first_elem + D.nelem - 1) finalize_launch(p, D, cin, s_out, cin.count + base + mine_total, lane);
+    if (t == D.first_elem + D.nelem - 1) {
+      wait_previous_launch();  // the sentinels go to an index array the previous launch may write too
+      finalize_launch(p, D, cin, s_out, cin.count + base + mine_total, lane);
+    }
   }
 }
 
@@ -1176,10 +1204,17 @@ SJ_DEV void scan4_body(const sj_tensor_map *tmap, const ScanParams &p, uint8_t *
 #endif
   // the CTA's first ticket: the atomic's round trip overlaps the set-up below
   uint32_t first_ticket = 0;
-  if (tid == 0) first_ticket = sj_atomic_add(p.ticket, 1u);
+  unsigned long long t_entry = 0;
+  if (tid == 0) {
+    if (p.stamps != nullptr) t_entry = sj_globaltimer();
+    first_ticket = sj_atomic_add(p.ticket, 1u);
+  }
+  // the carry-in is the previous launch's carry-out; an input the previous launch writes must not be read before it is done
+  if (p.carry_in != nullptr || !p.early_input) wait_previous_launch();
   Carry cin;
   cin.count = 0; cin.state = 0; cin.ttable = 0; cin.flags = 0; cin.reserved = 0;
   if (p.carry_in != nullptr) cin = *p.carry_in;
+  if (tid == 0 && p.stamps != nullptr && first_ticket == 0) p.stamps[0] = t_entry;
   // ~140 mbarriers: one thread each (a single thread initialising them all is slow)
   if (tid < unsigned(kNS)) {
     sj_mbar_init(&S->ticket_ready[tid], 1);
@@ -1248,6 +1283,7 @@ SJ_DEV void scan4_body(const sj_tensor_map *tmap, const ScanParams &p, uint8_t *
     sj_threadfence();
     const uint32_t done = sj_atomic_add(p.ticket + 1, 1u);
     if (done == sj_nctas() - 1) {
+      wait_previous_launch();  // no launch completes before its predecessor: what follows on the stream relies on both being done
       p.ticket[0] = 0;
       p.ticket[1] = 0;
       p.ticket[2] = 0;
@@ -1274,6 +1310,7 @@ SJ_DEV void scan4_body(const sj_tensor_map *tmap, const ScanParams &p, uint8_t *
           sj_st_sys_u64(rec + 1, w1);
         }
       }
+      if (p.stamps != nullptr) p.stamps[1] = sj_globaltimer();
       sj_threadfence();
     }
   }

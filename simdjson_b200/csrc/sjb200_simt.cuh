@@ -35,11 +35,21 @@ struct CtaShared {
   pthread_barrier_t bar;
   uint8_t *smem;
 };
+// Programmatic dependent launch between emulated grids (tests/simt_emul_pdl.cpp): a grid's threads may run while its
+// predecessor still runs; sj_griddep_wait blocks until every thread of the predecessor has exited, and the harness
+// starts the successor once every CTA of this grid has triggered or exited.  Null: no predecessor, no successor.
+struct GridDep {
+  GridDep *prev = nullptr;
+  std::atomic<unsigned> running{0};   // threads of this grid that have not exited
+  std::atomic<unsigned> released{0};  // CTAs that have triggered or exited
+  std::atomic<uint8_t> *cta_released = nullptr;
+};
 struct ThreadCtx {
   unsigned tid = 0, cta = 0, nctas = 0;
   unsigned phase = 0;
   WarpShared *warp = nullptr;
   CtaShared *ctas = nullptr;
+  GridDep *dep = nullptr;
 };
 extern thread_local ThreadCtx tctx;
 
@@ -148,6 +158,19 @@ SJ_DEV unsigned long long sj_globaltimer() {
   return (unsigned long long)ts.tv_sec * 1000000000ull + (unsigned long long)ts.tv_nsec;
 }
 SJ_DEV uint32_t sj_clock32() { return uint32_t(sj_globaltimer()); }
+
+SJ_DEV void sj_griddep_wait() {
+  const simt::GridDep *d = simt::tctx.dep;
+  if (d == nullptr || d->prev == nullptr) return;
+  while (d->prev->running.load(std::memory_order_acquire) != 0) {
+    struct timespec ts = {0, 20000};
+    nanosleep(&ts, nullptr);
+  }
+}
+SJ_DEV void sj_griddep_launch_dependents() {
+  simt::GridDep *d = simt::tctx.dep;
+  if (d != nullptr && d->cta_released[simt::tctx.cta].exchange(1) == 0) d->released.fetch_add(1);
+}
 
 // ---- mbarrier with deferred TMA copies
 struct sj_tensor_map {  // what the emulated TMA needs to know about the 2-D uint8 [rows][128] tensor
@@ -313,6 +336,11 @@ SJ_DEV unsigned long long sj_globaltimer() {
   return t;
 }
 SJ_DEV uint32_t sj_clock32() { return uint32_t(clock64()); }  // SM-local cycle counter (cheap; for intervals on one SM)
+// Programmatic dependent launch.  wait: until the grids this one depends on have completed and their memory is visible
+// (returns at once in a grid launched without the attribute).  launch_dependents: this CTA lets the next grid on the
+// stream start (the first call of a CTA counts; a CTA that exits without it counts at its exit).
+SJ_DEV void sj_griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+SJ_DEV void sj_griddep_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
 typedef CUtensorMap sj_tensor_map;
 typedef unsigned long long sj_mbar_t;
