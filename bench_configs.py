@@ -481,7 +481,8 @@ def run_check(args, rank, world, total=256 << 20):
     second exchange round and re-scans, through the real plumbing (CUDA IPC windows; NCCL for the handles).  Every rank
     compares its base + indexes with the oracle's scan of the whole prefix.  Then sharded minify on the same buffer and
     cuts (every rank's kept bytes at its base in the oracle's minify of the whole buffer) and sharded validate_utf8 on
-    random UTF-8 cut at character boundaries, valid and with one corrupted byte: one JSON line each.  With one process
+    random UTF-8 cut at character boundaries, valid and with one corrupted byte, and sharded RS-delimited and
+    comma-delimited passes (modes 3-6) on the rows written as both kinds of stream: one JSON line each.  With one process
     (no torchrun) the ranks run as threads of this process on one GPU."""
     torch, dist, sj, dev, local = _setup(rank, world)
     from simdjson_b200 import corpus, sharding
@@ -570,7 +571,75 @@ def run_check(args, rank, world, total=256 << 20):
         print(json.dumps({"check": "sharded validate_utf8, AND of the shards' verdicts",
                           "result": {"ranks": nranks, "bytes": len(text), "cuts": "character boundaries (sjb200_shard_cut)", "processes": world,
                                      "verdicts": {"valid": verdicts[0], "one corrupted byte": verdicts[1]}, "ok": bool(ok_u)}}), flush=True)
-    return bool(ok and ok_m and ok_u)
+    ok_d = _check_delimited(torch, dist, sj, sharding, dev, local, rank, world, nranks, O, port, corpus, total // 8)
+    return bool(ok and ok_m and ok_u and ok_d)
+
+
+def _delimited_cuts(O, port, raw, nranks, rs):
+    """cuts of a delimited stream, cycling through: inside a separator run (RS) or right after a root comma (comma),
+    inside a string value (the rank behind it re-scans), and at an arbitrary character boundary"""
+    from simdjson_b200 import sharding
+    a = np.frombuffer(raw, dtype=np.uint8)
+    cuts = list(sharding.shard_cuts(a, nranks))
+    for k in range(1, nranks):
+        pos, lim = cuts[k], cuts[k + 1]
+        if k % 3 == 1:
+            hit = raw.find(b"\x1e \x1e" if rs else b",\n", pos, lim)
+            if hit > 0:
+                cuts[k] = hit + 1  # RS: between the run's first RS and its whitespace; comma: right after the root comma
+        elif k % 3 == 2:
+            for _ in range(64):
+                hit = raw.find(b',"', pos, lim)
+                if hit < 0 or hit + 3 >= lim:
+                    break
+                cand = hit + 2
+                row0 = raw.rfind(b"\n", 0, cand) + 1
+                if B.raw_scan(O, port, a[row0:cand], 0)[1] & 2:  # bit 1: in a string
+                    cuts[k] = cand
+                    break
+                pos = hit + 1
+    return cuts
+
+
+def _check_delimited(torch, dist, sj, sharding, dev, local, rank, world, nranks, O, port, corpus, size):
+    """sharded RS-delimited (RS run before every row, some runs of several RS) and comma-delimited (rows joined by a root
+    comma and a line feed) passes in every delimited mode: every rank checks its error code, n, its kept filtered
+    entries at their global position and the three tail words against the oracle's stage1 of the whole stream; the
+    filtered_before of every rank must be the prefix sum of the filtered counts"""
+    rows = [r for r in bytes(corpus.ndjson_rows(size)).split(b"\n") if r]
+    streams = {"rs": b"".join((b"\x1e \x1e\n" if i % 5 == 0 else b"\x1e") + r + b"\n" for i, r in enumerate(rows)), "comma": b",\n".join(rows)}
+    ok_all = True
+    for kind, raw in streams.items():
+        cuts = _delimited_cuts(O, port, raw, nranks, kind == "rs")
+        a = np.frombuffer(raw, dtype=np.uint8)
+        modes = (3, 4) if kind == "rs" else (5, 6)
+        result = {"ranks": nranks, "bytes": len(raw), "processes": world,
+                  "cuts": ("inside separator runs" if kind == "rs" else "right after root commas") + ", inside strings, arbitrary"}
+        for mode in modes:
+            want = port.stage1(a, mode)
+
+            def body(r, comm, parser, d, stream, want=want, mode=mode, cuts=cuts):
+                d_idx = torch.empty(int(sj.lib().sjb200_index_words(d.numel())), dtype=torch.int32, device=dev)
+                rc, x = comm.scan_delimited(d, d_idx, r == nranks - 1, mode, stream)
+                torch.cuda.synchronize()
+                if rc != want.err or int(x.stream.bytes_before) != cuts[r]:
+                    return (False, 0, 0, 0, 0)
+                n, kept, fb = int(x.stream.n), int(x.stream.kept), int(x.filtered_before)
+                good = True
+                if want.wrote:
+                    got = (d_idx[:kept].cpu().numpy().view(np.uint32) + np.uint32(cuts[r])).astype(np.uint32)
+                    good = (n == want.n and kept == min(max(n - fb, 0), int(x.filtered)) and np.array_equal(got, want.idx[fb: fb + kept])
+                            and [int(t) for t in x.tail] == [int(w) for w in want.idx[n: n + 3]])
+                return good, int(x.filtered), fb, int(x.stream.shard.rescanned), kept
+            good, infos = _sharded_ranks(torch, dist, sj, sharding, dev, local, rank, world, nranks, lambda r: a[cuts[r]: cuts[r + 1]], body)
+            good = good and all(infos[r][2] == sum(i[1] for i in infos[:r]) for r in range(nranks))
+            good = good and (not want.wrote or sum(i[4] for i in infos) == want.n)  # the kept entries are the first n
+            ok_all = ok_all and good
+            result[f"mode{mode}"] = {"error": int(want.err), "n": int(want.n) if want.wrote else None, "rescans": sum(i[3] for i in infos), "ok": bool(good)}
+        if rank == 0:
+            print(json.dumps({"check": f"sharded {'RS-delimited' if kind == 'rs' else 'comma-delimited'} stage 1 (modes {modes[0]}-{modes[1]}), "
+                              "the filters carried across the cuts", "result": result}), flush=True)
+    return ok_all
 
 
 def _sharded_ranks(torch, dist, sj, sharding, dev, local, rank, world, nranks, shard_of, body):

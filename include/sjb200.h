@@ -279,8 +279,8 @@ SJB200_API int sjb200_validate_utf8_sharded(sjb200_comm *comm, const uint8_t *d_
 
 /* stage 1 of a whitespace-separated stream (NDJSON, concatenated documents) sharded the same way, with the whole
  * stream's finish(): `mode` is SJB200_REGULAR, SJB200_STREAMING_PARTIAL or SJB200_STREAMING_FINAL (3-6, the RS and
- * comma-delimited streams, are rejected with UNEXPECTED_ERROR: their filters need bracket depth and separator runs carried
- * across the cuts).  Every rank passes the same mode; last_shard = 1 on the last rank only.  In the streaming modes the
+ * comma-delimited streams, are rejected with UNEXPECTED_ERROR: they go through sjb200_stage1_sharded_delimited, whose
+ * result describes a compacted array).  Every rank passes the same mode; last_shard = 1 on the last rank only.  In the streaming modes the
  * last shard alone is trimmed of a partial UTF-8 character at its end (a shard that trims to nothing still takes part).
  * Cuts at character boundaries (sjb200_shard_cut / sjb200_shard_cut_line).  A stream pass has its own kind, so a rank
  * whose peers enqueued another kind for the same pass fails with UNEXPECTED_ERROR.
@@ -313,6 +313,39 @@ SJB200_API int sjb200_stage1_sharded_stream_enqueue(sjb200_comm *comm, const uin
 SJB200_API int sjb200_stage1_sharded_stream_finish(sjb200_comm *comm, sjb200_sharded_stream_result *out);
 SJB200_API int sjb200_stage1_sharded_stream(sjb200_comm *comm, const uint8_t *d_shard, size_t len, int last_shard, int mode, uint32_t *d_idx,
                                  sjb200_sharded_stream_result *out, void *stream);
+
+/* stage 1 of an RS-delimited (RFC 7464, modes SJB200_JSON_SEQUENCE_*) or comma-delimited (SJB200_COMMA_DELIMITED_*)
+ * stream sharded the same way, with the whole stream's filter and finish().  `mode` is 3..6 (0-2 are rejected with
+ * UNEXPECTED_ERROR: use sjb200_stage1_sharded_stream).  Same rules as that call: every rank passes the same mode,
+ * last_shard = 1 on the last rank only, cuts at character boundaries, only the last shard is trimmed of a partial UTF-8
+ * character (a shard that trims to nothing still takes part).  A delimited pass has its own kind: a rank whose peers
+ * enqueued another kind for the same pass fails with UNEXPECTED_ERROR.
+ *
+ * finish returns, on every rank, the error code stage1(whole buffer, mode) returns, and:
+ *   stream.n      that call's n_structural_indexes (0 where it leaves n untouched);
+ *   filtered      this shard's entries after the filter: d_idx[0, filtered), shard-relative, in stream order;
+ *   filtered_before  the filtered entries of all earlier ranks (the global position of d_idx[0]);
+ *   stream.kept   how many of them are among the first n (d_idx[0, kept) + bytes_before);
+ *   stream.bytes_before, stream.total_bytes, stream.first_starts_document  as for sjb200_stage1_sharded_stream, over the
+ *                 filtered array (so sjb200_document_table_shard_dev works unchanged on d_idx[0, kept));
+ *   tail          the whole call's index words n, n+1, n+2 (absolute, uint32): the next batch start (partial modes) or
+ *                 the stream's length (final modes), then what the reference's in-place filter leaves behind.
+ * Gathered as G = concat over ranks of (d_idx[0, kept) + bytes_before) (mod 2^32), followed by tail[0..2], G[0, n + 3)
+ * is the whole call's index array up to n + 3.  The words of d_idx past `filtered` are unspecified.
+ * Three host-synchronised rounds follow the scan's: a carry round (bracket depth / separator run entering each shard), a
+ * filter round (filter counts, last separator, the walks of find_next_document_index) and a tail round. */
+typedef struct {
+  sjb200_sharded_stream_result stream;  /* n, kept count entries of the FILTERED array */
+  uint64_t filtered;
+  uint64_t filtered_before;
+  uint32_t tail[3];
+  uint32_t reserved;
+} sjb200_sharded_delimited_result;
+SJB200_API int sjb200_stage1_sharded_delimited_enqueue(sjb200_comm *comm, const uint8_t *d_shard, size_t len, int last_shard, int mode, uint32_t *d_idx,
+                                            void *stream);
+SJB200_API int sjb200_stage1_sharded_delimited_finish(sjb200_comm *comm, sjb200_sharded_delimited_result *out);
+SJB200_API int sjb200_stage1_sharded_delimited(sjb200_comm *comm, const uint8_t *d_shard, size_t len, int last_shard, int mode, uint32_t *d_idx,
+                                    sjb200_sharded_delimited_result *out, void *stream);
 
 /* the document starts of one shard of a sharded stream pass: (local structural index, shard-relative byte) pairs of
  * d_idx[0, kept), structural 0 counted when first_starts_document says so (both from the pass's result).  A rank's
@@ -353,6 +386,40 @@ typedef struct {
 /* final_state / flags_all as in sjb200_sharded_result.  Returns res->error. */
 SJB200_API int sjb200_stream_fold(int mode, int nranks, uint32_t final_state, uint32_t flags_all, const sjb200_stream_summary *sums,
                        sjb200_stream_fold_result *res, sjb200_stream_rank *ranks /* nranks */);
+
+/* the host fold of a delimited pass's filter round, pure: what every rank's finish computes.  Per shard: */
+typedef struct {
+  uint64_t count;         /* structurals of the shard's scan (after the second round) */
+  uint32_t len;           /* shard length after the trim */
+  uint32_t filtered;      /* entries its filter kept (with the carried-in depth / run) */
+  uint32_t seps;          /* separators it counted: RS bytes of the runs of RS entries, or root commas */
+  uint32_t last_sep;      /* shard-relative byte of the last one (seps > 0) */
+  uint32_t below;         /* filtered entries before last_sep (seps > 0) */
+  uint32_t reserved;
+  sjb200_stream_summary walk;        /* the stream summary of the filtered entries (count is ignored) */
+  sjb200_stream_summary walk_below;  /* the same of the first `below` of them (comma-delimited partial mode) */
+} sjb200_delimited_summary;
+typedef struct {
+  uint64_t kept;
+  uint64_t filtered_before;
+  uint64_t bytes_before;
+  uint32_t first_starts_document;
+  uint32_t reserved;
+} sjb200_delimited_rank;
+typedef struct {
+  int error;
+  uint32_t n_written;       /* 0: n left untouched */
+  uint64_t n;
+  uint64_t total_bytes;
+  /* the words n, n+1, n+2: tail_rank[k] < 0: the word is tail_val[k]; else rank tail_rank[k] holds it at local position
+   * tail_pos[k] of its filtered entries (tail_filtered[k] = 1) or of its scanned structurals (0), shard-relative */
+  int32_t tail_rank[3];
+  uint32_t tail_pos[3];
+  uint32_t tail_filtered[3];
+  uint32_t tail_val[3];
+} sjb200_delimited_fold_result;
+SJB200_API int sjb200_delimited_fold(int mode, int nranks, uint32_t final_state, uint32_t flags_all, const sjb200_delimited_summary *sums,
+                          sjb200_delimited_fold_result *res, sjb200_delimited_rank *ranks /* nranks */);
 
 /* fold: state entering shard r given the ttables of shards 0..r-1 and the document's initial state 0 */
 SJB200_API uint32_t sjb200_fold_state(const uint32_t *ttables, int nshards_before);

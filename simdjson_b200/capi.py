@@ -26,6 +26,7 @@ EXPORTS = [
     "sjb200_tokens_dev", "sjb200_string_buf_capacity",
     "sjb200_stage1_sharded_stream", "sjb200_stage1_sharded_stream_enqueue", "sjb200_stage1_sharded_stream_finish",
     "sjb200_document_table_shard_dev", "sjb200_stream_fold",
+    "sjb200_stage1_sharded_delimited", "sjb200_stage1_sharded_delimited_enqueue", "sjb200_stage1_sharded_delimited_finish", "sjb200_delimited_fold",
 ]
 COMM_HANDLE_BYTES = 64
 
@@ -74,6 +75,26 @@ class StreamRank(C.Structure):
 
 class StreamFoldResult(C.Structure):
     _fields_ = [("error", C.c_int), ("n_written", C.c_uint32), ("n", C.c_uint64), ("total_bytes", C.c_uint64)]
+
+
+class ShardedDelimitedResult(C.Structure):
+    _fields_ = [("stream", ShardedStreamResult), ("filtered", C.c_uint64), ("filtered_before", C.c_uint64), ("tail", C.c_uint32 * 3),
+                ("reserved", C.c_uint32)]
+
+
+class DelimitedSummary(C.Structure):
+    _fields_ = [("count", C.c_uint64), ("len", C.c_uint32), ("filtered", C.c_uint32), ("seps", C.c_uint32), ("last_sep", C.c_uint32),
+                ("below", C.c_uint32), ("reserved", C.c_uint32), ("walk", StreamSummary), ("walk_below", StreamSummary)]
+
+
+class DelimitedRank(C.Structure):
+    _fields_ = [("kept", C.c_uint64), ("filtered_before", C.c_uint64), ("bytes_before", C.c_uint64), ("first_starts_document", C.c_uint32),
+                ("reserved", C.c_uint32)]
+
+
+class DelimitedFoldResult(C.Structure):
+    _fields_ = [("error", C.c_int), ("n_written", C.c_uint32), ("n", C.c_uint64), ("total_bytes", C.c_uint64), ("tail_rank", C.c_int32 * 3),
+                ("tail_pos", C.c_uint32 * 3), ("tail_filtered", C.c_uint32 * 3), ("tail_val", C.c_uint32 * 3)]
 
 
 def load():
@@ -138,6 +159,11 @@ def load():
         "sjb200_document_table_shard_dev": (C.c_int, [vp, vp, vp, C.c_uint32, C.c_int, vp, C.c_uint32, u32p, vp]),
         "sjb200_stream_fold": (C.c_int, [C.c_int, C.c_int, C.c_uint32, C.c_uint32, C.POINTER(StreamSummary), C.POINTER(StreamFoldResult),
                                          C.POINTER(StreamRank)]),
+        "sjb200_stage1_sharded_delimited": (C.c_int, [vp, vp, sz, C.c_int, C.c_int, vp, C.POINTER(ShardedDelimitedResult), vp]),
+        "sjb200_stage1_sharded_delimited_enqueue": (C.c_int, [vp, vp, sz, C.c_int, C.c_int, vp, vp]),
+        "sjb200_stage1_sharded_delimited_finish": (C.c_int, [vp, C.POINTER(ShardedDelimitedResult)]),
+        "sjb200_delimited_fold": (C.c_int, [C.c_int, C.c_int, C.c_uint32, C.c_uint32, C.POINTER(DelimitedSummary), C.POINTER(DelimitedFoldResult),
+                                            C.POINTER(DelimitedRank)]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)

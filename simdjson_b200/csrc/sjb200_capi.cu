@@ -1386,7 +1386,10 @@ struct sjb200_comm {
   unsigned long long *peer[kMaxRanks] = {};        // peer[r] = rank r's window as seen from this device
   bool opened[kMaxRanks] = {};                     // mapped through cudaIpcOpenMemHandle (to be closed)
   bool connected = false;
-  unsigned long long *h_rec = nullptr;             // pinned [kMaxRanks][kSumWords]: records ([r][0..1]) or summaries
+  unsigned long long *h_rec = nullptr;             // pinned [kMaxRanks][kDelimWords]: records ([r][0..1]), summaries or delimited blocks
+  uint32_t *h_tot = nullptr;                       // pinned [4]: a delimited pass's filter totals
+  uint32_t *d_scratch = nullptr;                   // a delimited pass's filter scratch (delim_scratch_words)
+  size_t scratch_words = 0;
   Carry *d_result = nullptr;                       // [kXchgSteps] the launches' own result blocks
   cudaStream_t poll_stream = nullptr;
   cudaEvent_t done[kXchgSteps] = {};
@@ -1400,12 +1403,15 @@ constexpr size_t kWindowWords = kXchgWindowWords;
 uint32_t window_slot(uint32_t seq, int round) { return (seq % uint32_t(kXchgSteps)) * 2u + uint32_t(round); }
 
 // wait (host polling, bounded) until every rank's record of (seq, round) is in the local window; records -> comm->h_rec.
-// round 2: the summaries of a streaming pass (kSumWords words per rank, each tagged with seq).
-int comm_collect(sjb200_comm *m, uint32_t seq, int round) {
+// round 2: the summaries of a streaming pass (kSumWords words per rank, each tagged with seq).  round 3: words
+// [first, first + nwords) of every rank's delimited block (h_rec[r * kDelimWords + k], the whole blocks are copied).
+int comm_collect(sjb200_comm *m, uint32_t seq, int round, int first = 0, int nwords = 0) {
   sjb200_ctx *c = m->ctx;
-  const bool sums = (round == 2);
-  const unsigned long long *src = sums ? m->window + xchg_summary_at(seq, 0) : m->window + size_t(window_slot(seq, round)) * kMaxRanks * 2;
-  const size_t words = sums ? size_t(kSumWords) : 2;
+  const bool sums = (round == 2), delim = (round == 3);
+  const unsigned long long *src = delim  ? m->window + xchg_delim_at(seq, 0)
+                                  : sums ? m->window + xchg_summary_at(seq, 0)
+                                         : m->window + size_t(window_slot(seq, round)) * kMaxRanks * 2;
+  const size_t words = delim ? size_t(kDelimWords) : sums ? size_t(kSumWords) : 2;
   const auto t0 = std::chrono::steady_clock::now();
   for (;;) {
     if (!ok(c, cudaMemcpyAsync(m->h_rec, src, size_t(m->nranks) * words * 8, cudaMemcpyDeviceToHost, m->poll_stream), "D2H window") ||
@@ -1414,6 +1420,10 @@ int comm_collect(sjb200_comm *m, uint32_t seq, int round) {
     c->xchg_polls++;
     bool all = true;
     for (int r = 0; r < m->nranks; r++) {
+      if (delim) {
+        for (int k = first; k < first + nwords; k++) all = all && uint32_t(m->h_rec[size_t(r) * kDelimWords + k] >> 32) == seq;
+        continue;
+      }
       if (!sums) { all = all && xchg_complete(m->h_rec[2 * r], m->h_rec[2 * r + 1], seq); continue; }
       for (int k = 0; k < kSumWords; k++) all = all && uint32_t(m->h_rec[size_t(r) * kSumWords + k] >> 32) == seq;
     }
@@ -1440,9 +1450,10 @@ extern "C" int sjb200_comm_create(sjb200_ctx *c, int rank, int nranks, sjb200_co
   bool good = dev_alloc(c, &m->window, kWindowWords, "cudaMalloc(window)") &&
               ok(c, cudaMemset(m->window, 0, kWindowWords * sizeof(unsigned long long)), "memset window") &&
               dev_alloc(c, &m->d_result, kXchgSteps, "cudaMalloc(results)") &&
-              ok(c, cudaMallocHost(&hp, kMaxRanks * kSumWords * 8), "cudaMallocHost") &&
+              ok(c, cudaMallocHost(&hp, kMaxRanks * kDelimWords * 8 + 16), "cudaMallocHost") &&
               ok(c, cudaStreamCreateWithFlags(&m->poll_stream, cudaStreamNonBlocking), "stream");
   m->h_rec = static_cast<unsigned long long *>(hp);
+  if (hp) m->h_tot = reinterpret_cast<uint32_t *>(m->h_rec + kMaxRanks * kDelimWords);
   for (int i = 0; good && i < kXchgSteps; i++) good = ok(c, cudaEventCreateWithFlags(&m->done[i], cudaEventDisableTiming), "event");
   if (!good) { sjb200_comm_destroy(m); return SJB200_MEMALLOC; }
   m->peer[rank] = m->window;
@@ -1457,7 +1468,7 @@ extern "C" void sjb200_comm_destroy(sjb200_comm *m) {
   cudaDeviceSynchronize();
   for (int r = 0; r < kMaxRanks; r++)
     if (m->opened[r] && m->peer[r]) cudaIpcCloseMemHandle(m->peer[r]);
-  cudaFree(m->window); cudaFree(m->d_result);
+  cudaFree(m->window); cudaFree(m->d_result); cudaFree(m->d_scratch);
   if (m->h_rec) cudaFreeHost(m->h_rec);
   if (m->poll_stream) cudaStreamDestroy(m->poll_stream);
   for (auto e : m->done) if (e) cudaEventDestroy(e);
@@ -1513,22 +1524,23 @@ namespace {
 // window; m->done[slot] marks the end of the launch on `stream`.
 int sharded_enqueue(sjb200_comm *m, int kind, const uint8_t *d_shard, size_t len, int last_shard, uint32_t *d_idx, uint8_t *d_dst, void *stream,
                     int mode = SJB200_REGULAR) {
-  const bool idx_kind = (kind == kIndex || kind == kStream);
+  const bool idx_kind = (kind == kIndex || kind == kStream || kind == kDelim);
   if (!m || !m->connected || !d_shard || len == 0 || len > kMaxBytes || (idx_kind && !d_idx) || (kind == kMinify && !d_dst))
     return SJB200_UNEXPECTED_ERROR;
   if (kind == kStream && (mode < SJB200_REGULAR || mode > SJB200_STREAMING_FINAL)) return SJB200_UNEXPECTED_ERROR;
+  if (kind == kDelim && (mode < SJB200_JSON_SEQUENCE_PARTIAL || mode > SJB200_COMMA_DELIMITED_FINAL)) return SJB200_UNEXPECTED_ERROR;
   if (m->head - m->tail >= uint32_t(kXchgSteps / 2)) return SJB200_CAPACITY;  // too many passes in flight: finish some first
   sjb200_ctx *c = m->ctx;
   DeviceGuard g(c->device);
   const auto t_enq = std::chrono::steady_clock::now();
   cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
-  if (kind == kStream && last_shard && mode != SJB200_REGULAR) {  // the partial UTF-8 trim of the stream's end (json_structural_indexer.h L198-204)
+  if ((kind == kStream || kind == kDelim) && last_shard && mode != SJB200_REGULAR) {  // the partial UTF-8 trim of the stream's end (json_structural_indexer.h L198-204)
     const size_t k = std::min<size_t>(3, len);
     if (!ok(c, cudaMemcpyAsync(c->h_small, d_shard + len - k, k, cudaMemcpyDeviceToHost, s), "D2H tail") || !ok(c, cudaStreamSynchronize(s), "sync"))
       return SJB200_UNEXPECTED_ERROR;
     len = trim_partial_utf8_tail(c->h_small, k, len);
   }
-  const int scan_kind = idx_kind ? kIndex : kind;  // a stream pass scans like stage 1; only its record's kind differs
+  const int scan_kind = idx_kind ? kIndex : kind;  // stream and delimited passes scan like stage 1; only their records' kind differs
   if (use_scan4(c, scan_kind) && len && !ensure_desc(c, len)) return SJB200_MEMALLOC;
   const uint32_t seq = m->head + 1;  // tags start at 1: a zeroed window never matches
   XchgTarget x;
@@ -1660,6 +1672,16 @@ int sharded_finish(sjb200_comm *m, int kind, sjb200_sharded_result *out) {
   return SJB200_SUCCESS;
 }
 
+// the kSumWords words of stream_summary_kernel (sjb200_params.h) -> the fold's summary of `count` structurals
+void decode_summary(const unsigned long long *w, uint64_t count, sjb200_stream_summary *out) {
+  sjb200_stream_summary &s = *out;
+  s.count = count;
+  s.len = uint32_t(w[0]); s.first_byte = uint32_t(w[1]); s.last_byte = uint32_t(w[2]);
+  s.start_index = uint32_t(w[3]); s.start_byte = uint32_t(w[4]);
+  s.net_obj = int32_t(uint32_t(w[5])); s.net_arr = int32_t(uint32_t(w[6]));
+  s.role_first = uint32_t(w[7]) & 7u; s.role_last = (uint32_t(w[7]) >> 3) & 7u; s.has_start = (uint32_t(w[7]) >> 6) & 1u;
+}
+
 // Complete the oldest pass in flight, a stream pass: the scan's fold (sharded_finish), then the summary round and the
 // host fold of the whole stream's finish() (sjb200_stream_fold), then this rank's sentinels and rewrites.
 int sharded_stream_finish(sjb200_comm *m, sjb200_sharded_stream_result *out) {
@@ -1684,22 +1706,15 @@ int sharded_stream_finish(sjb200_comm *m, sjb200_sharded_stream_result *out) {
   memset(&x, 0, sizeof(x));
   for (int r = 0; r < kMaxRanks; r++) x.xchg_peer[r] = m->peer[r];
   x.xchg_nranks = uint32_t(m->nranks); x.xchg_rank = uint32_t(m->rank); x.xchg_seq = st.seq;
-  if (!ok(c, launch_stream_summary(st.d_buf, st.d_idx, uint32_t(my_count), uint32_t(kept), uint32_t(st.len), st.mode != SJB200_REGULAR, x, m->poll_stream),
+  if (!ok(c, launch_stream_summary(st.d_buf, st.d_idx, uint32_t(my_count), uint32_t(kept), uint32_t(st.len), st.mode != SJB200_REGULAR, x,
+                                   xchg_summary_at(st.seq, uint32_t(m->rank)), m->poll_stream),
           "stream summary"))
     return SJB200_UNEXPECTED_ERROR;
   c->launches++;
   rc = comm_collect(m, st.seq, 2);
   if (rc != SJB200_SUCCESS) return rc;
   sjb200_stream_summary sums[kMaxRanks];
-  for (int r = 0; r < m->nranks; r++) {
-    const unsigned long long *w = m->h_rec + size_t(r) * kSumWords;
-    sjb200_stream_summary &s = sums[r];
-    s.count = counts[r];
-    s.len = uint32_t(w[0]); s.first_byte = uint32_t(w[1]); s.last_byte = uint32_t(w[2]);
-    s.start_index = uint32_t(w[3]); s.start_byte = uint32_t(w[4]);
-    s.net_obj = int32_t(uint32_t(w[5])); s.net_arr = int32_t(uint32_t(w[6]));
-    s.role_first = uint32_t(w[7]) & 7u; s.role_last = (uint32_t(w[7]) >> 3) & 7u; s.has_start = (uint32_t(w[7]) >> 6) & 1u;
-  }
+  for (int r = 0; r < m->nranks; r++) decode_summary(m->h_rec + size_t(r) * kSumWords, counts[r], &sums[r]);
   sjb200_stream_fold_result res;
   sjb200_stream_rank ranks[kMaxRanks];
   const int err = sjb200_stream_fold(st.mode, m->nranks, out->shard.final_state, out->shard.flags_all, sums, &res, ranks);
@@ -1719,6 +1734,117 @@ int sharded_stream_finish(sjb200_comm *m, sjb200_sharded_stream_result *out) {
       return SJB200_UNEXPECTED_ERROR;
     c->launches += (sentinels ? 1 : 0) + (me.nrewrites ? 1 : 0);
   }
+  return err;
+}
+}  // namespace
+
+// Complete the oldest pass in flight, a delimited pass (modes 3..6): the scan's fold (sharded_finish), then three rounds,
+// each a small kernel storing tagged words into every rank's window and a comm_collect (DESIGN.md section 5):
+//   carry   every rank's length and the bracket net (comma) or "ends inside a separator run" / "whitespace / RS only"
+//           (RS) -> this rank's depth_in / run_in;
+//   filter  the filter of sjb200_docs.cu with that carry, into the scratch, then its totals and the walks of
+//           find_next_document_index over the filtered entries -> sjb200_delimited_fold;
+//   tail    the holders of the words n, n+1, n+2 publish them (skipped when the fold knows all three); then the
+//           filtered entries go back into d_idx.
+namespace {
+int sharded_delimited_finish(sjb200_comm *m, sjb200_sharded_delimited_result *out) {
+  if (!m || !out || m->tail == m->head) return SJB200_UNEXPECTED_ERROR;
+  memset(out, 0, sizeof(*out));
+  const sjb200_comm::Step st = m->steps[m->tail % uint32_t(kXchgSteps)];
+  int rc = sharded_finish(m, kDelim, &out->stream.shard);
+  if (rc != SJB200_SUCCESS) return rc;  // (an internal error is seen by every rank alike: nobody runs the extra rounds)
+  sjb200_ctx *c = m->ctx;
+  DeviceGuard g(c->device);
+  const int me = m->rank;
+  uint64_t counts[kMaxRanks];
+  int holder = -1;  // the rank that holds the stream's last structural
+  for (int r = 0; r < m->nranks; r++) {
+    counts[r] = xchg_count(m->h_rec[2 * r]);
+    if (counts[r]) holder = r;
+  }
+  const bool unclosed = (out->stream.shard.final_state >> 1) & 1u;
+  const bool comma = (st.mode == SJB200_COMMA_DELIMITED_PARTIAL || st.mode == SJB200_COMMA_DELIMITED_FINAL);
+  const bool walk_below = (st.mode == SJB200_COMMA_DELIMITED_PARTIAL);
+  // the structurals this shard's filter considers: less the stream's last one when it ends inside a string
+  const uint32_t n = uint32_t(counts[me]) - ((unclosed && holder == me) ? 1u : 0u);
+  const uint32_t len = uint32_t(st.len);
+  const size_t need = delim_scratch_words(n);
+  if (m->scratch_words < need) {
+    cudaFree(m->d_scratch); m->d_scratch = nullptr; m->scratch_words = 0;
+    if (!dev_alloc(c, &m->d_scratch, need, "cudaMalloc(delimited scratch)")) return SJB200_MEMALLOC;
+    m->scratch_words = need;
+  }
+  ScanParams x;
+  memset(&x, 0, sizeof(x));
+  for (int r = 0; r < kMaxRanks; r++) x.xchg_peer[r] = m->peer[r];
+  x.xchg_nranks = uint32_t(m->nranks); x.xchg_rank = uint32_t(me); x.xchg_seq = st.seq;
+  const size_t at = xchg_delim_at(st.seq, uint32_t(me));
+  cudaStream_t s = m->poll_stream;
+  // carry round
+  if (!ok(c, launch_delim_carry(st.d_buf, st.d_idx, n, len, comma, m->d_scratch, x, at + kDelimCarryAt, s), "delimited carry")) return SJB200_UNEXPECTED_ERROR;
+  c->launches++;
+  if ((rc = comm_collect(m, st.seq, 3, kDelimCarryAt, kDelimCarryWords)) != SJB200_SUCCESS) return rc;
+  uint32_t lens[kMaxRanks];
+  int depth = 0, depth_in = 0;
+  bool run = false, run_in = false;  // run: the bytes from an RS entry of an earlier shard up to here are whitespace / RS
+  for (int r = 0; r < m->nranks; r++) {
+    const unsigned long long *w = m->h_rec + size_t(r) * kDelimWords + kDelimCarryAt;
+    lens[r] = uint32_t(w[0]);
+    if (r == me) { depth_in = depth; run_in = run; }
+    if (comma) depth += int32_t(uint32_t(w[1]));
+    else run = uint32_t(w[1]) != 0 || (run && uint32_t(w[2]) != 0);
+  }
+  // filter round
+  if (!ok(c, launch_delim_filter(st.d_buf, len, st.d_idx, n, comma, depth_in, run_in, m->d_scratch, m->h_tot, s), "delimited filter") ||
+      !ok(c, cudaStreamSynchronize(s), "sync"))
+    return SJB200_UNEXPECTED_ERROR;
+  const uint32_t filtered = m->h_tot[0], below = m->h_tot[3];
+  const uint32_t *dst = delim_filtered(m->d_scratch);
+  if (!ok(c, launch_stream_summary(st.d_buf, dst, filtered, filtered, len, 1, x, at + kDelimWalkAt, s), "delimited walk") ||
+      (walk_below && !ok(c, launch_stream_summary(st.d_buf, dst, below, below, len, 1, x, at + kDelimWalkBelowAt, s), "delimited walk")) ||
+      !ok(c, launch_delim_publish_totals(m->d_scratch, n, x, at + kDelimTotalsAt, s), "delimited totals"))
+    return SJB200_UNEXPECTED_ERROR;
+  c->launches += 6 + (walk_below ? 1 : 0);
+  const int upto = walk_below ? kDelimTailAt : kDelimWalkBelowAt;
+  if ((rc = comm_collect(m, st.seq, 3, kDelimTotalsAt, upto - kDelimTotalsAt)) != SJB200_SUCCESS) return rc;
+  sjb200_delimited_summary sums[kMaxRanks];
+  memset(sums, 0, sizeof(sums));
+  for (int r = 0; r < m->nranks; r++) {
+    const unsigned long long *w = m->h_rec + size_t(r) * kDelimWords;
+    sjb200_delimited_summary &d = sums[r];
+    d.count = counts[r]; d.len = lens[r];
+    d.filtered = uint32_t(w[kDelimTotalsAt]); d.seps = uint32_t(w[kDelimTotalsAt + 1]);
+    d.last_sep = uint32_t(w[kDelimTotalsAt + 2]); d.below = uint32_t(w[kDelimTotalsAt + 3]);
+    decode_summary(w + kDelimWalkAt, d.filtered, &d.walk);
+    if (walk_below) decode_summary(w + kDelimWalkBelowAt, d.below, &d.walk_below);
+  }
+  sjb200_delimited_fold_result res;
+  sjb200_delimited_rank ranks[kMaxRanks];
+  const int err = sjb200_delimited_fold(st.mode, m->nranks, out->stream.shard.final_state, out->stream.shard.flags_all, sums, &res, ranks);
+  out->stream.n = res.n;
+  out->stream.kept = ranks[me].kept;
+  out->stream.bytes_before = ranks[me].bytes_before;
+  out->stream.total_bytes = res.total_bytes;
+  out->stream.first_starts_document = ranks[me].first_starts_document;
+  out->filtered = filtered;
+  out->filtered_before = ranks[me].filtered_before;
+  // tail round
+  DelimTail t;
+  memset(&t, 0, sizeof(t));
+  t.add = uint32_t(ranks[me].bytes_before);
+  bool publish = false;
+  for (int k = 0; k < 3; k++) {
+    if (res.tail_rank[k] < 0) continue;
+    publish = true;
+    if (res.tail_rank[k] == me) { t.src[k] = res.tail_filtered[k] ? 1 : 2; t.pos[k] = res.tail_pos[k]; }
+  }
+  if (!ok(c, launch_delim_tail(m->d_scratch, n, st.d_idx, t, publish, x, at + kDelimTailAt, s), "delimited tail") ||
+      !ok(c, cudaStreamSynchronize(s), "sync"))
+    return SJB200_UNEXPECTED_ERROR;
+  c->launches += publish ? 2 : 1;
+  if (publish && (rc = comm_collect(m, st.seq, 3, kDelimTailAt, 3)) != SJB200_SUCCESS) return rc;
+  for (int k = 0; k < 3; k++)
+    out->tail[k] = res.tail_rank[k] < 0 ? res.tail_val[k] : uint32_t(m->h_rec[size_t(res.tail_rank[k]) * kDelimWords + kDelimTailAt + k]);
   return err;
 }
 }  // namespace
@@ -1846,6 +1972,140 @@ extern "C" int sjb200_stream_fold(int mode, int nranks, uint32_t final_state, ui
   res->n = m;
   if (m == 0) return done(SJB200_EMPTY);
   return done(utf8 ? SJB200_UTF8_ERROR : SJB200_SUCCESS);
+}
+
+extern "C" int sjb200_stage1_sharded_delimited_enqueue(sjb200_comm *m, const uint8_t *d_shard, size_t len, int last_shard, int mode, uint32_t *d_idx,
+                                                       void *stream) {
+  return sharded_enqueue(m, kDelim, d_shard, len, last_shard, d_idx, nullptr, stream, mode);
+}
+
+extern "C" int sjb200_stage1_sharded_delimited_finish(sjb200_comm *m, sjb200_sharded_delimited_result *out) { return sharded_delimited_finish(m, out); }
+
+extern "C" int sjb200_stage1_sharded_delimited(sjb200_comm *m, const uint8_t *d_shard, size_t len, int last_shard, int mode, uint32_t *d_idx,
+                                               sjb200_sharded_delimited_result *out, void *stream) {
+  int rc = sjb200_stage1_sharded_delimited_enqueue(m, d_shard, len, last_shard, mode, d_idx, stream);
+  if (rc != SJB200_SUCCESS) return rc;
+  return sjb200_stage1_sharded_delimited_finish(m, out);
+}
+
+// The fold of a delimited pass's filter round into the whole stream's finish() for modes 3..6 (json_structural_indexer.h
+// L344-396 with find_next_document_index_json_sequence / filter_comma_delimited, as filter_finish_kernel runs it on one
+// GPU).  The filtered entries are sorted across the ranks, so the global last separator is the last one of the last
+// rank that counted any, and the entries before it are the filtered entries of the ranks before plus its `below`.
+// find_next_document_index over the first k filtered entries is sjb200_stream_fold's walk over the ranks' walk
+// summaries (every rank's full walk, the last rank's walk_below when k ends at its `below`).  The words after n are those
+// of the array the reference's in-place filter leaves: the filtered entries, then the scan's structurals, then the
+// sentinels len, len, 0.
+extern "C" int sjb200_delimited_fold(int mode, int nranks, uint32_t final_state, uint32_t flags_all, const sjb200_delimited_summary *sums,
+                                     sjb200_delimited_fold_result *res, sjb200_delimited_rank *ranks) {
+  if (!res || !ranks || !sums || nranks < 1 || nranks > kMaxRanks || mode < SJB200_JSON_SEQUENCE_PARTIAL || mode > SJB200_COMMA_DELIMITED_FINAL)
+    return SJB200_UNEXPECTED_ERROR;
+  memset(res, 0, sizeof(*res));
+  memset(ranks, 0, sizeof(*ranks) * size_t(nranks));
+  uint64_t base[kMaxRanks], off = 0, T = 0, W = 0, seps = 0;
+  int sep_rank = -1;  // the last rank that counted a separator
+  for (int r = 0; r < nranks; r++) {
+    ranks[r].bytes_before = off;
+    ranks[r].filtered_before = W;
+    off += sums[r].len;
+    base[r] = T;
+    T += sums[r].count;
+    W += sums[r].filtered;
+    seps += sums[r].seps;
+    if (sums[r].seps) sep_rank = r;
+  }
+  const uint64_t L = off;
+  res->total_bytes = L;
+  for (int k = 0; k < 3; k++) res->tail_rank[k] = -1;
+  const bool rs = (mode == SJB200_JSON_SEQUENCE_PARTIAL || mode == SJB200_JSON_SEQUENCE_FINAL);
+  const bool is_final = (mode == SJB200_JSON_SEQUENCE_FINAL || mode == SJB200_COMMA_DELIMITED_FINAL);
+  const bool unclosed = (final_state >> 1) & 1u;
+  auto word = [&](int k, uint64_t p) {  // word p of the array after the in-place filter -> tail k
+    if (p < W || p < T) {
+      const bool f = p < W;
+      int r = 0;
+      while (!(f ? (p >= ranks[r].filtered_before && p < ranks[r].filtered_before + sums[r].filtered) : (p >= base[r] && p < base[r] + sums[r].count))) r++;
+      res->tail_rank[k] = r;
+      res->tail_pos[k] = uint32_t(p - (f ? ranks[r].filtered_before : base[r]));
+      res->tail_filtered[k] = f ? 1u : 0u;
+    } else {
+      res->tail_val[k] = p < T + 2 ? uint32_t(L) : 0u;
+    }
+  };
+  auto words_from = [&](uint64_t p) { for (int k = 0; k < 3; k++) word(k, p + uint64_t(k)); };
+  auto done = [&](int err) {
+    res->error = err;
+    for (int r = 0; r < nranks && res->n_written; r++) {
+      const uint64_t k = res->n > ranks[r].filtered_before ? res->n - ranks[r].filtered_before : 0;
+      ranks[r].kept = std::min<uint64_t>(k, sums[r].filtered);
+    }
+    for (int r = 0, prev = -1; r < nranks; r++) {  // prev: the last earlier shard with kept entries
+      if (ranks[r].kept == 0) continue;
+      ranks[r].first_starts_document = (prev < 0) ? 1u : uint32_t(starts_document(sums[r].walk.role_first, sums[prev].walk.role_last));
+      prev = r;
+    }
+    return err;
+  };
+  // find_next_document_index over the first k filtered entries
+  auto walk = [&](uint64_t k) -> uint64_t {
+    sjb200_stream_summary ws[kMaxRanks];
+    for (int r = 0; r < nranks; r++) {
+      const uint64_t fb = ranks[r].filtered_before;
+      const uint64_t cnt = std::min<uint64_t>(k > fb ? k - fb : 0, sums[r].filtered);
+      if (cnt == 0) memset(&ws[r], 0, sizeof(ws[r]));
+      else ws[r] = (cnt == sums[r].filtered) ? sums[r].walk : sums[r].walk_below;
+      ws[r].count = cnt;
+      ws[r].len = sums[r].len;
+    }
+    sjb200_stream_fold_result fr;
+    sjb200_stream_rank fk[kMaxRanks];
+    sjb200_stream_fold(SJB200_STREAMING_FINAL, nranks, 0, 0, ws, &fr, fk);
+    return fr.n;
+  };
+  if (flags_all & kFlagInternal) return done(SJB200_UNEXPECTED_ERROR);
+  if (L == 0) return done(SJB200_UTF8_ERROR);                        // L198-204: nothing left after the trim
+  if (flags_all & kFlagCtl) return done(SJB200_UNESCAPED_CHARS);    // L261-263
+  res->n_written = 1;
+  res->n = T;
+  if (T == 0) { words_from(0); return done(SJB200_EMPTY); }          // L289-291
+  if (!is_final && unclosed && T == 1) { res->n = 0; words_from(0); return done(SJB200_CAPACITY); }  // L298-302, before the filter
+  uint64_t m = 0, n_res = W, next_start = L;
+  bool too_large = false;
+  const uint64_t last_sep = sep_rank >= 0 ? ranks[sep_rank].bytes_before + sums[sep_rank].last_sep : 0;
+  const uint64_t before_sep = sep_rank >= 0 ? ranks[sep_rank].filtered_before + sums[sep_rank].below : 0;
+  if (W != 0) {
+    if (rs) {
+      if (seps == 0) m = is_final ? walk(W) : 0;
+      else if (is_final) m = W;
+      else {
+        next_start = last_sep;
+        if (seps < 2) too_large = true;
+        else m = before_sep;
+      }
+    } else {
+      if (is_final) m = walk(W);
+      else if (seps == 0) too_large = true;
+      else {
+        next_start = last_sep + 1;
+        if (before_sep != 0) { n_res = before_sep; m = walk(before_sep); }
+      }
+    }
+  }
+  if (!is_final) {  // L344-359, L367-384
+    if (too_large) { res->n = n_res; words_from(n_res); return done(SJB200_CAPACITY); }
+    if (m == 0) { res->n = 0; words_from(0); return done(SJB200_EMPTY); }
+    res->n = m;
+    res->tail_val[0] = uint32_t(next_start);
+    word(1, m + 1);
+    word(2, m + 2);
+  } else {  // L360-366, L385-393: word m + 1 = the old word m
+    res->n = m;
+    res->tail_val[0] = uint32_t(L);
+    word(1, m);
+    word(2, m + 2);
+    if (m == 0) return done(SJB200_EMPTY);
+  }
+  return done((flags_all & kFlagUtf8) ? SJB200_UTF8_ERROR : SJB200_SUCCESS);
 }
 
 extern "C" int sjb200_stage1_sharded_enqueue(sjb200_comm *m, const uint8_t *d_shard, size_t len, int last_shard, uint32_t *d_idx, void *stream) {

@@ -161,10 +161,10 @@ __global__ void __launch_bounds__(kFinishThreads) stream_finish_kernel(const uin
 
 // The summary of one shard for the extra round of a sharded streaming pass: walk back from the shard's last kept
 // structural to its last internal document start (index >= 1), then store the kSumWords-word summary (sjb200_params.h)
-// into every rank's window.  kept = the shard's structurals, less the stream's last one when the stream ends inside a
-// string and this shard holds it; walk = 0 (regular mode) skips the walk.
+// into every rank's window at word `at` (this rank's block).  kept = the shard's structurals, less the stream's last one
+// when the stream ends inside a string and this shard holds it; walk = 0 (regular mode) skips the walk.
 __global__ void __launch_bounds__(kFinishThreads) stream_summary_kernel(const uint8_t *buf, const uint32_t *idx, uint32_t count, uint32_t kept, uint32_t len,
-                                                                       int walk, ScanParams x) {
+                                                                       int walk, ScanParams x, size_t at) {
   __shared__ int sh[kFinishThreads / 32];
   int start = -1, nobj = 0, narr = 0;
   if (walk && kept > 0) last_document_start(buf, idx, kept, sh, &start, &nobj, &narr);
@@ -179,7 +179,7 @@ __global__ void __launch_bounds__(kFinishThreads) stream_summary_kernel(const ui
     w[5] = uint32_t(nobj);
     w[6] = uint32_t(narr);
     w[7] = (kept ? role_of(buf[idx[0]]) | (role_of(buf[idx[kept - 1]]) << 3) : 0u) | (start >= 0 ? 1u << 6 : 0u);
-    unsigned long long *rec = x.xchg_peer[r] + xchg_summary_at(x.xchg_seq, x.xchg_rank);
+    unsigned long long *rec = x.xchg_peer[r] + at;
     for (int k = 0; k < kSumWords; k++) {
       const unsigned long long v = (static_cast<unsigned long long>(x.xchg_seq) << 32) | w[k];
       asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(rec + k), "l"(v) : "memory");
@@ -359,18 +359,23 @@ __global__ void __launch_bounds__(1024) int_scan_kernel(int *v, uint32_t count, 
 
 // What structural i contributes to the filtered array: 0 or 1 entries (value in *out).  RS format: RS entries go; the
 // leader of a run "RS (ws | RS)*" counts the run's separators and, when a scalar is glued to the run's end (stage 1 sees
-// RS as a scalar byte, so that value has no index of its own), contributes the value's position.
-__device__ __forceinline__ int rs_entry(const uint8_t *buf, uint32_t len, const uint32_t *idx, uint32_t n, uint32_t i, uint32_t *out, uint32_t *seps,
-                                        uint32_t *last_sep) {
+// RS as a scalar byte, so that value has no index of its own), contributes the value's position.  lead_end (a shard of a
+// sharded pass entered inside a separator run of an earlier shard, else 0): the end of the shard's leading whitespace /
+// RS run, found by the lead step of filter_pass_kernel, which also counts that run; the RS entries before it are
+// absorbed.  A shard's walk stops at its end (len); the shard where the run ends adds the scalar glued to it.
+__device__ __forceinline__ bool ws_or_rs(uint32_t c) { return is_ws(c) || c == 0x1E; }
+__device__ __forceinline__ int rs_entry(const uint8_t *buf, uint32_t len, const uint32_t *idx, uint32_t n, uint32_t i, uint32_t lead_end, uint32_t *out,
+                                        uint32_t *seps, uint32_t *last_sep) {
   const uint32_t at = idx[i];
   if (buf[at] != 0x1E) { *out = at; return 1; }
+  if (i == 0 && at < lead_end) return 0;  // (a later RS of the leading run follows an absorbed one: the check below)
   if (i > 0 && buf[idx[i - 1]] == 0x1E) {  // inside the run an earlier RS entry leads?
     bool same = true;
     for (uint32_t q = idx[i - 1] + 1; q < at && same; q++) same = is_ws(buf[q]) || buf[q] == 0x1E;
     if (same) return 0;
   }
   uint32_t s = 1, last = at, v = at + 1;
-  while (v < len && (is_ws(buf[v]) || buf[v] == 0x1E)) {
+  while (v < len && ws_or_rs(buf[v])) {
     if (buf[v] == 0x1E) { s++; last = v; }
     v++;
   }
@@ -383,15 +388,33 @@ __device__ __forceinline__ int rs_entry(const uint8_t *buf, uint32_t len, const 
   }
   return 0;
 }
+// the lead step of a shard entered inside a run (run_in): the separators of its leading run and the scalar glued to the
+// run's end, unless the shard's scan emitted that byte; *lead_end = the run's end.  One thread walks the run, like the
+// leader walk of a run inside a shard.
+__device__ __forceinline__ int rs_lead(const uint8_t *buf, uint32_t len, const uint32_t *idx, uint32_t n, uint32_t *out, uint32_t *seps, uint32_t *last_sep,
+                                       uint32_t *lead_end) {
+  uint32_t v = 0;
+  for (; v < len && ws_or_rs(buf[v]); v++)
+    if (buf[v] == 0x1E) { (*seps)++; *last_sep = max(*last_sep, v); }
+  *lead_end = v;
+  if (v < len && role_of(buf[v]) == kRoleValue) {
+    uint32_t j = 0;
+    while (j < n && idx[j] < v) j++;
+    if (!(j < n && idx[j] == v)) { *out = v; return 1; }
+  }
+  return 0;
+}
 
 struct FilterTotals {
   uint32_t kept, seps, last_sep, reserved;
 };
 
-// pass A (count) and pass B (write) share the per-thread walk; kComma selects the format
+// pass A (count) and pass B (write) share the per-thread walk; kComma selects the format.  depth_in / run_in: what a
+// shard of a sharded pass carries in from the shards before it (0 for a whole stream)
 template <bool kComma, bool kWrite>
 __global__ void __launch_bounds__(kFltThreads) filter_pass_kernel(const uint8_t *buf, uint32_t len, const uint32_t *idx, uint32_t n, const int *tile_depth,
-                                                                 int *tile_count /* A: out; B: exclusive offsets */, uint32_t *dst, FilterTotals *totals) {
+                                                                 int *tile_count /* A: out; B: exclusive offsets */, uint32_t *dst, FilterTotals *totals,
+                                                                 int depth_in, int run_in) {
   __shared__ int sh[kFltThreads / 32 + 1];
   const uint32_t first = blockIdx.x * kFltTile + threadIdx.x * kFltPerThread;
   int depth = 0;
@@ -402,11 +425,13 @@ __global__ void __launch_bounds__(kFltThreads) filter_pass_kernel(const uint8_t 
       if (i < n) { const uint32_t r = role_of(buf[idx[i]]); d += net_obj(r) + net_arr(r); }
     }
     int total;
-    depth = tile_depth[blockIdx.x] + block_excl_scan(d, sh, &total);
+    depth = depth_in + tile_depth[blockIdx.x] + block_excl_scan(d, sh, &total);
   }
-  uint32_t vals[kFltPerThread];
+  uint32_t vals[kComma ? kFltPerThread : kFltPerThread + 1];  // (RS: one more for the lead step)
   int cnt = 0;
   uint32_t seps = 0, last_sep = 0;
+  uint32_t lead_end = 0;  // (the thread of structural 0 does the lead step; no other thread reads lead_end)
+  if (!kComma && run_in && first == 0 && rs_lead(buf, len, idx, n, &vals[0], &seps, &last_sep, &lead_end)) cnt = 1;
   for (int k = 0; k < kFltPerThread; k++) {
     const uint32_t i = first + k;
     if (i >= n) break;
@@ -418,7 +443,7 @@ __global__ void __launch_bounds__(kFltThreads) filter_pass_kernel(const uint8_t 
       vals[cnt++] = at;
     } else {
       uint32_t v = 0;
-      if (rs_entry(buf, len, idx, n, i, &v, &seps, &last_sep)) vals[cnt++] = v;
+      if (rs_entry(buf, len, idx, n, i, lead_end, &v, &seps, &last_sep)) vals[cnt++] = v;
     }
   }
   int total;
@@ -489,6 +514,89 @@ __global__ void __launch_bounds__(kFinishThreads) filter_finish_kernel(const uin
   }
 }
 
+// ---------------------------------------------------------------------------------------------- sharded RS / comma passes
+// the extra rounds of a delimited pass (sjb200_capi.cu): every kernel stores its words, tagged with x.xchg_seq, into
+// every rank's window at word `at` (this rank's block, sjb200_params.h)
+__device__ __forceinline__ void store_tagged(const ScanParams &x, uint32_t r, size_t at, const uint32_t *w, int nwords) {
+  unsigned long long *rec = x.xchg_peer[r] + at;
+  for (int k = 0; k < nwords; k++) {
+    const unsigned long long v = (static_cast<unsigned long long>(x.xchg_seq) << 32) | w[k];
+    asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(rec + k), "l"(v) : "memory");
+  }
+}
+
+// RS carry round, over the whole grid: *other = 1 when a byte after the shard's last structural (byte 0 without one) is
+// neither whitespace nor RS.  Threads leave at the first such byte they meet, the others at their next look at *other,
+// so a shard that ends in a long string or scalar costs a few strides, one that ends in a long whitespace run one pass.
+constexpr int kWsThreads = 256, kWsBlocks = 528, kWsPoll = 16;
+__global__ void __launch_bounds__(kWsThreads) trailing_ws_kernel(const uint8_t *buf, const uint32_t *idx, uint32_t n, uint32_t len, int *other) {
+  const uint64_t lo = n ? uint64_t(idx[n - 1]) + 1 : 0u, stride = uint64_t(gridDim.x) * blockDim.x;
+  uint32_t k = 0;
+  for (uint64_t q = lo + uint64_t(blockIdx.x) * blockDim.x + threadIdx.x; q < len; q += stride) {
+    if (!ws_or_rs(buf[q])) { atomicOr(other, 1); return; }
+    if (++k % kWsPoll == 0 && *reinterpret_cast<volatile int *>(other)) return;
+  }
+}
+
+// carry round: the shard's length and what the filters of later shards need from it -- comma: the bracket net over its n
+// structurals (*depth_total); RS: whether it ends inside a separator run (its last structural is an RS entry followed
+// only by whitespace / RS, *other == 0) and whether it is whitespace / RS only
+__global__ void delim_carry_kernel(const uint8_t *buf, const uint32_t *idx, uint32_t n, uint32_t len, int comma, const int *depth_total, const int *other,
+                                   ScanParams x, size_t at) {
+  const bool ok = comma || *other == 0;
+  if (threadIdx.x < x.xchg_nranks) {
+    uint32_t w[kDelimCarryWords];
+    w[0] = len;
+    w[1] = comma ? uint32_t(*depth_total) : uint32_t(n > 0 && buf[idx[n - 1]] == 0x1E && ok);
+    w[2] = comma ? 0u : uint32_t(n == 0 && ok);
+    store_tagged(x, threadIdx.x, at, w, kDelimCarryWords);
+  }
+}
+
+// filter round: {filtered entries, separators, last separator, filtered entries before it} -> out4
+__global__ void delim_totals_kernel(const uint32_t *dst, const int *kept_total, const FilterTotals *tot, uint32_t *out4) {
+  if (threadIdx.x != 0) return;
+  const uint32_t n = uint32_t(*kept_total), seps = tot->seps, last_sep = tot->last_sep;
+  uint32_t lo = 0, hi = seps ? n : 0u;
+  while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (dst[mid] < last_sep) lo = mid + 1; else hi = mid; }
+  out4[0] = n; out4[1] = seps; out4[2] = last_sep; out4[3] = lo;
+}
+
+__global__ void publish_kernel(const uint32_t *src, uint32_t nwords, ScanParams x, size_t at) {
+  if (threadIdx.x < x.xchg_nranks) store_tagged(x, threadIdx.x, at, src, int(nwords));
+}
+
+// tail round: the (at most three) words n, n+1, n+2 of the whole call this rank holds, read before the filtered entries
+// go back into idx -- a word past the filtered array is what the scan left there (a raw structural, as after the
+// reference's in-place filter)
+__global__ void delim_tail_kernel(const uint32_t *dst, const uint32_t *idx, DelimTail t, ScanParams x, size_t at) {
+  uint32_t w[3];
+  for (int k = 0; k < 3; k++) w[k] = t.src[k] == 1 ? dst[t.pos[k]] + t.add : (t.src[k] == 2 ? idx[t.pos[k]] + t.add : 0u);
+  if (threadIdx.x < x.xchg_nranks) store_tagged(x, threadIdx.x, at, w, 3);
+}
+
+struct FilterScratch {
+  uint32_t *dst;
+  int *tile_depth, *tile_count;
+  FilterTotals *tot;
+  int *kept_total, *depth_total, *other;
+  uint32_t *out4;
+};
+// the scratch of launch_stream_filter (n + 8 words, the two tile arrays, the totals), then the delimited rounds' words
+FilterScratch filter_layout(uint32_t *scratch, uint32_t n) {
+  const uint32_t ntiles = (n + kFltTile - 1) / kFltTile;
+  FilterScratch f;
+  f.dst = scratch;
+  f.tile_depth = reinterpret_cast<int *>(scratch + size_t(n) + 8);
+  f.tile_count = f.tile_depth + ntiles + 4;
+  f.tot = reinterpret_cast<FilterTotals *>(f.tile_count + ntiles + 4);
+  f.kept_total = reinterpret_cast<int *>(f.tot + 1);
+  f.depth_total = f.kept_total + 1;
+  f.other = f.kept_total + 2;
+  f.out4 = reinterpret_cast<uint32_t *>(f.kept_total + 4);
+  return f;
+}
+
 }  // namespace
 
 size_t filter_scratch_words(uint32_t n) { return size_t(n) + 8 + 2 * (size_t((n + kFltTile - 1) / kFltTile) + 4) + 8; }
@@ -510,13 +618,13 @@ cudaError_t launch_stream_filter(const uint8_t *buf, uint32_t len, uint32_t *idx
     if (comma) {
       comma_depth_kernel<<<ntiles, kFltThreads, 0, stream>>>(buf, idx, n, tile_depth);
       int_scan_kernel<<<1, 1024, 0, stream>>>(tile_depth, ntiles, nullptr);
-      filter_pass_kernel<true, false><<<ntiles, kFltThreads, 0, stream>>>(buf, len, idx, n, tile_depth, tile_count, dst, tot);
+      filter_pass_kernel<true, false><<<ntiles, kFltThreads, 0, stream>>>(buf, len, idx, n, tile_depth, tile_count, dst, tot, 0, 0);
       int_scan_kernel<<<1, 1024, 0, stream>>>(tile_count, ntiles, kept_total);
-      filter_pass_kernel<true, true><<<ntiles, kFltThreads, 0, stream>>>(buf, len, idx, n, tile_depth, tile_count, dst, tot);
+      filter_pass_kernel<true, true><<<ntiles, kFltThreads, 0, stream>>>(buf, len, idx, n, tile_depth, tile_count, dst, tot, 0, 0);
     } else {
-      filter_pass_kernel<false, false><<<ntiles, kFltThreads, 0, stream>>>(buf, len, idx, n, tile_depth, tile_count, dst, tot);
+      filter_pass_kernel<false, false><<<ntiles, kFltThreads, 0, stream>>>(buf, len, idx, n, tile_depth, tile_count, dst, tot, 0, 0);
       int_scan_kernel<<<1, 1024, 0, stream>>>(tile_count, ntiles, kept_total);
-      filter_pass_kernel<false, true><<<ntiles, kFltThreads, 0, stream>>>(buf, len, idx, n, tile_depth, tile_count, dst, tot);
+      filter_pass_kernel<false, true><<<ntiles, kFltThreads, 0, stream>>>(buf, len, idx, n, tile_depth, tile_count, dst, tot, 0, 0);
     }
     // only the kept entries go back: the words behind them keep what the scan left there, like the reference's in-place filter
     copy_kept_kernel<<<std::min<uint32_t>(ntiles, 1024u), 256, 0, stream>>>(idx, dst, kept_total);
@@ -544,8 +652,68 @@ cudaError_t launch_doc_table(const uint8_t *buf, const uint32_t *idx, uint32_t n
 }
 
 cudaError_t launch_stream_summary(const uint8_t *buf, const uint32_t *idx, uint32_t count, uint32_t kept, uint32_t len, int walk, const ScanParams &x,
-                                  cudaStream_t stream) {
-  stream_summary_kernel<<<1, kFinishThreads, 0, stream>>>(buf, idx, count, kept, len, walk, x);
+                                  size_t at, cudaStream_t stream) {
+  stream_summary_kernel<<<1, kFinishThreads, 0, stream>>>(buf, idx, count, kept, len, walk, x, at);
+  return cudaGetLastError();
+}
+
+size_t delim_scratch_words(uint32_t n) { return filter_scratch_words(n) + 8; }
+
+cudaError_t launch_delim_carry(const uint8_t *buf, const uint32_t *idx, uint32_t n, uint32_t len, bool comma, uint32_t *scratch, const ScanParams &x,
+                               size_t at, cudaStream_t stream) {
+  const FilterScratch f = filter_layout(scratch, n);
+  const uint32_t ntiles = (n + kFltTile - 1) / kFltTile;
+  if (comma) {
+    cudaError_t e = cudaMemsetAsync(f.tile_depth, 0, sizeof(int), stream);  // (the filter round's one tile when n = 0)
+    if (e == cudaSuccess) e = cudaMemsetAsync(f.depth_total, 0, sizeof(int), stream);
+    if (e != cudaSuccess) return e;
+    if (ntiles) {  // the tile depths stay in the scratch for the filter round
+      comma_depth_kernel<<<ntiles, kFltThreads, 0, stream>>>(buf, idx, n, f.tile_depth);
+      int_scan_kernel<<<1, 1024, 0, stream>>>(f.tile_depth, ntiles, f.depth_total);
+    }
+  } else {
+    cudaError_t e = cudaMemsetAsync(f.other, 0, sizeof(int), stream);
+    if (e != cudaSuccess) return e;
+    trailing_ws_kernel<<<kWsBlocks, kWsThreads, 0, stream>>>(buf, idx, n, len, f.other);
+  }
+  delim_carry_kernel<<<1, 32, 0, stream>>>(buf, idx, n, len, comma, f.depth_total, f.other, x, at);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_delim_filter(const uint8_t *buf, uint32_t len, const uint32_t *idx, uint32_t n, bool comma, int depth_in, bool run_in, uint32_t *scratch,
+                                uint32_t *totals_host, cudaStream_t stream) {
+  const FilterScratch f = filter_layout(scratch, n);
+  const uint32_t ntiles = std::max<uint32_t>(1u, (n + kFltTile - 1) / kFltTile);  // the lead step runs even without structurals
+  cudaError_t e = cudaMemsetAsync(f.tot, 0, sizeof(FilterTotals) + sizeof(int), stream);
+  if (e != cudaSuccess) return e;
+  if (comma) {
+    filter_pass_kernel<true, false><<<ntiles, kFltThreads, 0, stream>>>(buf, len, idx, n, f.tile_depth, f.tile_count, f.dst, f.tot, depth_in, 0);
+    int_scan_kernel<<<1, 1024, 0, stream>>>(f.tile_count, ntiles, f.kept_total);
+    filter_pass_kernel<true, true><<<ntiles, kFltThreads, 0, stream>>>(buf, len, idx, n, f.tile_depth, f.tile_count, f.dst, f.tot, depth_in, 0);
+  } else {
+    filter_pass_kernel<false, false><<<ntiles, kFltThreads, 0, stream>>>(buf, len, idx, n, f.tile_depth, f.tile_count, f.dst, f.tot, 0, run_in);
+    int_scan_kernel<<<1, 1024, 0, stream>>>(f.tile_count, ntiles, f.kept_total);
+    filter_pass_kernel<false, true><<<ntiles, kFltThreads, 0, stream>>>(buf, len, idx, n, f.tile_depth, f.tile_count, f.dst, f.tot, 0, run_in);
+  }
+  delim_totals_kernel<<<1, 32, 0, stream>>>(f.dst, f.kept_total, f.tot, f.out4);
+  e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  return cudaMemcpyAsync(totals_host, f.out4, 4 * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream);
+}
+
+const uint32_t *delim_filtered(const uint32_t *scratch) { return scratch; }
+
+cudaError_t launch_delim_publish_totals(uint32_t *scratch, uint32_t n, const ScanParams &x, size_t at, cudaStream_t stream) {
+  publish_kernel<<<1, 32, 0, stream>>>(filter_layout(scratch, n).out4, 4, x, at);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_delim_tail(uint32_t *scratch, uint32_t n, uint32_t *idx, const DelimTail &t, bool publish, const ScanParams &x, size_t at,
+                              cudaStream_t stream) {
+  const FilterScratch f = filter_layout(scratch, n);
+  if (publish) delim_tail_kernel<<<1, 32, 0, stream>>>(f.dst, idx, t, x, at);
+  const uint32_t ntiles = std::max<uint32_t>(1u, (n + kFltTile - 1) / kFltTile);
+  copy_kept_kernel<<<std::min<uint32_t>(ntiles + 1, 1024u), 256, 0, stream>>>(idx, f.dst, f.kept_total);
   return cudaGetLastError();
 }
 

@@ -18,8 +18,9 @@ constexpr int kXchgSteps = 64;                        // sharded passes whose ex
 #define SJB200_SCAN4_MIN_CTAS 2                       // CTAs per SM of the 8-scan-warp build of scan4
 #endif
 
-// ---- scan kinds (kStream: a stage-1 pass of the sharded streaming modes; it scans like kIndex, only its record differs)
-enum : int { kIndex = 0, kMinify = 1, kUtf8 = 2, kStream = 3 };
+// ---- scan kinds (kStream: a stage-1 pass of the sharded streaming modes; kDelim: one of the sharded RS / comma-delimited
+// modes.  Both scan like kIndex, only their records differ)
+enum : int { kIndex = 0, kMinify = 1, kUtf8 = 2, kStream = 3, kDelim = 4 };
 
 // Scanner state between consecutive launches of one document (chunked streaming,
 // multi-GPU shards).  state: bit0 escape, bit1 in_string, bit2 prev_scalar.
@@ -74,7 +75,7 @@ struct ScanParams {
   // with xchg_seq -- the path's one exchange step (SURVEY.md 8e) without a collective launch.  xchg_nranks == 0: no exchange.
   unsigned long long *xchg_peer[kMaxRanks];  // [r] = base of rank r's window: [slots][kMaxRanks][2] words
   uint32_t xchg_nranks, xchg_rank, xchg_slot, xchg_seq;
-  uint32_t xchg_kind;       // scan4 stage 1: the kind its record carries (kIndex, or kStream for a streaming pass)
+  uint32_t xchg_kind;       // scan4 stage 1: the kind its record carries (kIndex, kStream or kDelim)
   // scan4 stage 1, several whole documents in one launch: ndocs (1..kMaxLaunchDocs) entries in device memory.  buf, len,
   // use_tma, idx_out, carry_out and carry_out_host are then unused; tile_begin = 0, no carry-in, no exchange, pos_base = 0,
   // prev_word = 0x20202020, check_eof = write_sentinels = 1, and `flags` only collects what concerns the whole launch.
@@ -97,23 +98,25 @@ struct ScanParams {
 #endif
 // one shard record as two independently tagged 64-bit words (8-byte stores are single transactions):
 //   w0 = seq[30:0] << 33 | count[32:0]        w1 = seq << 32 | kind << 24 | flags << 16 | ttable << 8 | state_out
-// kind is the scan kind of the pass (kIndex 0, kMinify 1, kUtf8 2, kStream 3); count is structurals (kIndex, kStream),
-// kept bytes (kMinify) or 0 (kUtf8).
+// kind (3 bits, 24-26) is the scan kind of the pass (kIndex 0, kMinify 1, kUtf8 2, kStream 3, kDelim 4); count is
+// structurals (kIndex, kStream, kDelim), kept bytes (kMinify) or 0 (kUtf8).  Bit 26 was zero before kDelim existed, so the
+// records of the other kinds are unchanged.
 SJ_PARAMS_HD inline unsigned long long xchg_word0(uint32_t seq, uint64_t count) {
   return ((unsigned long long)(seq & 0x7FFFFFFFu) << 33) | (count & 0x1FFFFFFFFull);
 }
 SJ_PARAMS_HD inline unsigned long long xchg_word1(uint32_t seq, uint32_t state, uint32_t ttable, uint32_t flags, int kind) {
-  return ((unsigned long long)seq << 32) | ((unsigned long long)(uint32_t(kind) & 3u) << 24) | ((unsigned long long)(flags & 0xFFu) << 16) |
+  return ((unsigned long long)seq << 32) | ((unsigned long long)(uint32_t(kind) & 7u) << 24) | ((unsigned long long)(flags & 0xFFu) << 16) |
          ((unsigned long long)(ttable & 0x3Fu) << 8) | (state & 7u);
 }
-SJ_PARAMS_HD inline int xchg_kind(unsigned long long w1) { return int(uint32_t(w1 >> 24) & 3u); }
+SJ_PARAMS_HD inline int xchg_kind(unsigned long long w1) { return int(uint32_t(w1 >> 24) & 7u); }
 SJ_PARAMS_HD inline bool xchg_complete(unsigned long long w0, unsigned long long w1, uint32_t seq) {
   return uint32_t(w0 >> 33) == (seq & 0x7FFFFFFFu) && uint32_t(w1 >> 32) == seq;
 }
 SJ_PARAMS_HD inline uint64_t xchg_count(unsigned long long w0) { return w0 & 0x1FFFFFFFFull; }
 
 // The window: the records of the two rounds, [kXchgSteps][2][kMaxRanks][2] words, then the summary area of the streaming
-// passes' extra round, [kXchgSteps][kMaxRanks][kSumWords] words.  A summary is kSumWords words seq << 32 | payload:
+// passes' extra round, [kXchgSteps][kMaxRanks][kSumWords] words, then the area of the delimited passes' three extra
+// rounds, [kXchgSteps][kMaxRanks][kDelimWords] words (layout below).  A summary is kSumWords words seq << 32 | payload:
 //   0 shard length (after the trim)   1 byte of structural 0         2 byte of the last structural (kept or not)
 //   3 local index of the last internal document start   4 its byte  5 / 6 object / array bracket net (int32) from that
 //   start on, or over every kept structural when there is none
@@ -121,9 +124,22 @@ SJ_PARAMS_HD inline uint64_t xchg_count(unsigned long long w0) { return w0 & 0x1
 // (whether byte 0 is a structural is word 1 == 0 with a count > 0; the counts come from the records)
 constexpr int kSumWords = 8;
 constexpr size_t kXchgRecordWords = size_t(kXchgSteps) * 2 * kMaxRanks * 2;
-constexpr size_t kXchgWindowWords = kXchgRecordWords + size_t(kXchgSteps) * kMaxRanks * kSumWords;
+constexpr size_t kXchgSummaryWords = size_t(kXchgSteps) * kMaxRanks * kSumWords;
 SJ_PARAMS_HD inline size_t xchg_summary_at(uint32_t seq, uint32_t rank) {
   return kXchgRecordWords + (size_t(seq % uint32_t(kXchgSteps)) * kMaxRanks + rank) * kSumWords;
+}
+// A delimited pass's block of one rank, kDelimWords words, each seq << 32 | payload:
+//   carry round   0 shard length (after the trim)   1 comma: bracket net over the shard's structurals (int32); RS: the
+//                 shard ends inside a separator run   2 RS: the shard is whitespace / RS only
+//   filter round  4 filtered entries   5 separators   6 last separator (shard-relative)   7 filtered entries before it
+//                 8..15 the summary (as above) of the filtered entries   16..23 the same of the entries before the last
+//                 separator (comma-delimited partial mode only)
+//   tail round    24..26 the words n, n+1, n+2 of the whole call this rank holds (0 for the others)
+constexpr int kDelimWords = 32;
+enum : int { kDelimCarryAt = 0, kDelimCarryWords = 3, kDelimTotalsAt = 4, kDelimWalkAt = 8, kDelimWalkBelowAt = 16, kDelimTailAt = 24 };
+constexpr size_t kXchgWindowWords = kXchgRecordWords + kXchgSummaryWords + size_t(kXchgSteps) * kMaxRanks * kDelimWords;
+SJ_PARAMS_HD inline size_t xchg_delim_at(uint32_t seq, uint32_t rank) {
+  return kXchgRecordWords + kXchgSummaryWords + (size_t(seq % uint32_t(kXchgSteps)) * kMaxRanks + rank) * kDelimWords;
 }
 
 }  // namespace sjb200

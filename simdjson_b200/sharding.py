@@ -40,6 +40,31 @@ def fold_stream(mode, final_state, flags_all, summaries):
     return int(res.error), int(res.n_written), int(res.n), int(res.total_bytes), out
 
 
+def fold_delimited(mode, final_state, flags_all, summaries):
+    """sjb200_delimited_fold: summaries = one dict per shard with the fields of sjb200_delimited_summary, `walk` and
+    `walk_below` dicts with those of sjb200_stream_summary.  Returns (error, n_written, n, total_bytes, tail, [per rank
+    dict(kept, filtered_before, bytes_before, first_starts_document)]); tail = 3 entries, each ("value", word) or
+    ("filtered" | "scanned", rank, local position)"""
+    from . import capi
+    k = len(summaries)
+    sums = (capi.DelimitedSummary * k)()
+    for s, d in zip(sums, summaries):
+        for name, _ in capi.DelimitedSummary._fields_:
+            if name in ("walk", "walk_below"):
+                for f, _ in capi.StreamSummary._fields_:
+                    setattr(getattr(s, name), f, int(d.get(name, {}).get(f, 0)))
+            else:
+                setattr(s, name, int(d.get(name, 0)))
+    res = capi.DelimitedFoldResult()
+    ranks = (capi.DelimitedRank * k)()
+    _lib().sjb200_delimited_fold(int(mode), k, int(final_state), int(flags_all), sums, C.byref(res), ranks)
+    tail = [("value", int(res.tail_val[j])) if res.tail_rank[j] < 0 else
+            ("filtered" if res.tail_filtered[j] else "scanned", int(res.tail_rank[j]), int(res.tail_pos[j])) for j in range(3)]
+    out = [{"kept": int(r.kept), "filtered_before": int(r.filtered_before), "bytes_before": int(r.bytes_before),
+            "first_starts_document": int(r.first_starts_document)} for r in ranks]
+    return int(res.error), int(res.n_written), int(res.n), int(res.total_bytes), tail, out
+
+
 def shard_cuts(buf, nshards):
     """cut a host buffer into nshards byte ranges at UTF-8 character boundaries"""
     L = _lib()
@@ -173,8 +198,30 @@ class Comm:
             return rc, None
         return self.stream_finish()
 
+    # stage 1 of an RS-delimited (modes JSON_SEQUENCE_*) or comma-delimited (COMMA_DELIMITED_*) stream with the whole
+    # stream's filter and finish(); its passes share the window with the other kinds
+    def delimited_enqueue(self, d_shard, d_idx, last_shard, mode, stream=None):
+        from .implementation import _stream_ptr
+        return _lib().sjb200_stage1_sharded_delimited_enqueue(self._h, d_shard.data_ptr(), d_shard.numel(), int(last_shard), int(mode), d_idx.data_ptr(),
+                                                              _stream_ptr(stream))
+
+    def delimited_finish(self):
+        """(error_code, ShardedDelimitedResult): the error code and n of stage1(whole stream, mode) on every rank; this
+        shard's filtered entries d_idx[:filtered] (shard-relative), of which d_idx[:stream.kept] + stream.bytes_before are
+        among the first n; tail = the whole call's words n, n+1, n+2"""
+        res = self._capi.ShardedDelimitedResult()
+        rc = _lib().sjb200_stage1_sharded_delimited_finish(self._h, C.byref(res))
+        return rc, res
+
+    def scan_delimited(self, d_shard, d_idx, last_shard, mode, stream=None):
+        rc = self.delimited_enqueue(d_shard, d_idx, last_shard, mode, stream)
+        if rc != 0:
+            return rc, None
+        return self.delimited_finish()
+
     def document_table(self, d_shard, d_idx, result, stream=None):
-        """the document starts among this shard's kept structurals (result: a ShardedStreamResult): (local structural
+        """the document starts among this shard's kept structurals (result: a ShardedStreamResult, or the `stream` field of
+        a ShardedDelimitedResult, over the filtered entries): (local structural
         index, shard-relative byte) pairs as an int64 [ndocs, 2] CPU array.  Not collective."""
         import torch
 
