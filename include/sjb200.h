@@ -24,7 +24,7 @@
  *   sjb200_validate_utf8
  *        implementation::validate_utf8(buf,len)              include/simdjson/implementation.h L128
  * The *_dev variants take device pointers (input already resident in HBM); they are what the
- * roofline metric times.  The sharded variants (stage 1, minify, validate_utf8) are the per-GPU pieces of a multi-GPU
+ * roofline metric times.  The sharded variants (stage 1, minify, validate_utf8, stage-2-lite) are the per-GPU pieces of a multi-GPU
  * pass over one buffer cut by byte range (section 8e).
  */
 #ifndef SJB200_H
@@ -346,6 +346,44 @@ SJB200_API int sjb200_stage1_sharded_delimited_enqueue(sjb200_comm *comm, const 
 SJB200_API int sjb200_stage1_sharded_delimited_finish(sjb200_comm *comm, sjb200_sharded_delimited_result *out);
 SJB200_API int sjb200_stage1_sharded_delimited(sjb200_comm *comm, const uint8_t *d_shard, size_t len, int last_shard, int mode, uint32_t *d_idx,
                                     sjb200_sharded_delimited_result *out, void *stream);
+
+/* stage-2-lite (sjb200_tokens_dev) sharded the same way, on the same comm and window: every rank runs the token kernels
+ * on its shard, and the kernel that scans the string-buffer sums stores the shard's record and totals into every rank's
+ * window.  (d_idx, n) is a structural list of this shard from a sharded stage-1 pass (sjb200_stage1_sharded: count;
+ * stream and delimited passes: kept, over d_idx as that pass left it), state_in that pass's folded state_in, len the shard
+ * length it used (the last rank of a streaming pass: after the trim).  len and n may be 0.  A tokens pass has its own kind.
+ *
+ * The cut before a shard must be clean: state_in == 0 (the byte before it is whitespace, an operator or a closing quote),
+ * so that no token spans it.  Cuts after a raw line feed (sjb200_shard_cut_line) are clean for every input stage 1
+ * accepts without UNESCAPED_CHARS.  A token that spans a cut is detected, not handled: finish returns UNEXPECTED_ERROR.
+ *
+ * Outputs stay on their ranks, shard-relative: d_type[0, n), d_payload[0, n) and d_strbuf[0, string_bytes).  Gathered as
+ * the concatenations over the ranks of d_type, of d_payload with string_base added to '"' payloads and bytes_before to 'd'
+ * payloads, and of d_strbuf[0, string_bytes), they are byte-identical to sjb200_tokens_dev on the whole document (whose
+ * d_idx is the ranks' d_idx + bytes_before) when error is SUCCESS or a token error and short_ranks == 0.  Under CAPACITY
+ * each rank did what sjb200_tokens_dev does on its shard with its own strbuf_capacity.
+ *
+ * finish returns, on every rank alike: UNEXPECTED_ERROR when dirty_cuts != 0, when a peer enqueued another kind for the
+ * pass, or when a rank could not run its pass; else the error code of the first token in error in document order (the
+ * earliest rank's first), with first_error_index; else CAPACITY when some rank is short; else SUCCESS -- the precedence
+ * of sjb200_tokens_dev, where a token error wins over CAPACITY.  One host-synchronised round, no re-scan. */
+typedef struct {
+  int error;                  /* as returned */
+  uint32_t dirty_cuts;        /* bit r: rank r entered its shard with state_in != 0 */
+  uint32_t short_ranks;       /* bit r: rank r's string bytes exceed its strbuf_capacity (it wrote no records) */
+  uint32_t reserved;
+  uint64_t first_error_index; /* document-global structural index of the first token in error; UINT64_MAX if none */
+  uint64_t tokens_before;     /* n of all earlier ranks: token k here is token tokens_before + k of the document */
+  uint64_t bytes_before;      /* byte offset of this shard: a 'd' payload p is document offset bytes_before + p */
+  uint64_t n_strings, strings_before, total_strings;
+  uint64_t string_bytes, string_base, total_string_bytes; /* this rank's part of string_buf, its offset, the whole */
+} sjb200_sharded_tokens_result;
+SJB200_API int sjb200_tokens_sharded_enqueue(sjb200_comm *comm, const uint8_t *d_shard, size_t len, uint32_t state_in, const uint32_t *d_idx,
+                                  uint32_t n, uint8_t *d_type, uint64_t *d_payload, uint8_t *d_strbuf, size_t strbuf_capacity, void *stream);
+SJB200_API int sjb200_tokens_sharded_finish(sjb200_comm *comm, sjb200_sharded_tokens_result *out);
+SJB200_API int sjb200_tokens_sharded(sjb200_comm *comm, const uint8_t *d_shard, size_t len, uint32_t state_in, const uint32_t *d_idx, uint32_t n,
+                          uint8_t *d_type, uint64_t *d_payload, uint8_t *d_strbuf, size_t strbuf_capacity, sjb200_sharded_tokens_result *out,
+                          void *stream);
 
 /* the document starts of one shard of a sharded stream pass: (local structural index, shard-relative byte) pairs of
  * d_idx[0, kept), structural 0 counted when first_starts_document says so (both from the pass's result).  A rank's

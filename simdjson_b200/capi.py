@@ -27,6 +27,7 @@ EXPORTS = [
     "sjb200_stage1_sharded_stream", "sjb200_stage1_sharded_stream_enqueue", "sjb200_stage1_sharded_stream_finish",
     "sjb200_document_table_shard_dev", "sjb200_stream_fold",
     "sjb200_stage1_sharded_delimited", "sjb200_stage1_sharded_delimited_enqueue", "sjb200_stage1_sharded_delimited_finish", "sjb200_delimited_fold",
+    "sjb200_tokens_sharded", "sjb200_tokens_sharded_enqueue", "sjb200_tokens_sharded_finish",
 ]
 COMM_HANDLE_BYTES = 64
 
@@ -97,6 +98,13 @@ class DelimitedFoldResult(C.Structure):
                 ("tail_pos", C.c_uint32 * 3), ("tail_filtered", C.c_uint32 * 3), ("tail_val", C.c_uint32 * 3)]
 
 
+class ShardedTokensResult(C.Structure):
+    _fields_ = [("error", C.c_int), ("dirty_cuts", C.c_uint32), ("short_ranks", C.c_uint32), ("reserved", C.c_uint32),
+                ("first_error_index", C.c_uint64), ("tokens_before", C.c_uint64), ("bytes_before", C.c_uint64), ("n_strings", C.c_uint64),
+                ("strings_before", C.c_uint64), ("total_strings", C.c_uint64), ("string_bytes", C.c_uint64), ("string_base", C.c_uint64),
+                ("total_string_bytes", C.c_uint64)]
+
+
 def load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
@@ -164,6 +172,9 @@ def load():
         "sjb200_stage1_sharded_delimited_finish": (C.c_int, [vp, C.POINTER(ShardedDelimitedResult)]),
         "sjb200_delimited_fold": (C.c_int, [C.c_int, C.c_int, C.c_uint32, C.c_uint32, C.POINTER(DelimitedSummary), C.POINTER(DelimitedFoldResult),
                                             C.POINTER(DelimitedRank)]),
+        "sjb200_tokens_sharded": (C.c_int, [vp, vp, sz, C.c_uint32, vp, C.c_uint32, vp, vp, vp, sz, C.POINTER(ShardedTokensResult), vp]),
+        "sjb200_tokens_sharded_enqueue": (C.c_int, [vp, vp, sz, C.c_uint32, vp, C.c_uint32, vp, vp, vp, sz, vp]),
+        "sjb200_tokens_sharded_finish": (C.c_int, [vp, C.POINTER(ShardedTokensResult)]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)

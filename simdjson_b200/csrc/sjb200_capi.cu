@@ -1376,7 +1376,8 @@ extern "C" int sjb200_stage1_shard_dev_enqueue(sjb200_ctx *c, const uint8_t *d_b
 // shard with the speculated state 0; the scan kernel's last CTA stores the 16-byte record {count, state, transducer,
 // flags, kind} into every rank's window over NVLink -- no collective launch.  finish() reads the local window, folds the
 // true incoming state and base, and -- only when somebody's speculation was wrong -- re-scans and runs a second round.
-// A pass is stage 1, minify or validate_utf8 (its kind); passes of all kinds share the window and may be in flight
+// A pass is stage 1 (plain, stream or delimited), minify, validate_utf8 or stage-2-lite (its kind; the tokens pass's record
+// comes from tile_scan_kernel, sjb200_tape.cu); passes of all kinds share the window and may be in flight
 // together, up to kXchgSteps / 2 per rank (enqueue ... enqueue, finish ... finish), as long as every rank enqueues the
 // same sequence of kinds.
 struct sjb200_comm {
@@ -1391,6 +1392,10 @@ struct sjb200_comm {
   uint32_t *d_scratch = nullptr;                   // a delimited pass's filter scratch (delim_scratch_words)
   size_t scratch_words = 0;
   Carry *d_result = nullptr;                       // [kXchgSteps] the launches' own result blocks
+  // tokens passes, by the slot of their pass (a pass in flight keeps its own): totals, tile scratch (grow-only)
+  TokenTotals *d_tok_tot = nullptr;
+  void *d_tok_scratch[kXchgSteps] = {};
+  size_t tok_scratch_bytes[kXchgSteps] = {};
   cudaStream_t poll_stream = nullptr;
   cudaEvent_t done[kXchgSteps] = {};
   struct Step { const uint8_t *d_buf; size_t len; uint32_t *d_idx; uint8_t *d_dst; cudaStream_t stream; uint32_t seq; int last; int kind; int mode; } steps[kXchgSteps];
@@ -1468,7 +1473,8 @@ extern "C" void sjb200_comm_destroy(sjb200_comm *m) {
   cudaDeviceSynchronize();
   for (int r = 0; r < kMaxRanks; r++)
     if (m->opened[r] && m->peer[r]) cudaIpcCloseMemHandle(m->peer[r]);
-  cudaFree(m->window); cudaFree(m->d_result); cudaFree(m->d_scratch);
+  cudaFree(m->window); cudaFree(m->d_result); cudaFree(m->d_scratch); cudaFree(m->d_tok_tot);
+  for (void *p : m->d_tok_scratch) cudaFree(p);
   if (m->h_rec) cudaFreeHost(m->h_rec);
   if (m->poll_stream) cudaStreamDestroy(m->poll_stream);
   for (auto e : m->done) if (e) cudaEventDestroy(e);
@@ -1986,6 +1992,130 @@ extern "C" int sjb200_stage1_sharded_delimited(sjb200_comm *m, const uint8_t *d_
   int rc = sjb200_stage1_sharded_delimited_enqueue(m, d_shard, len, last_shard, mode, d_idx, stream);
   if (rc != SJB200_SUCCESS) return rc;
   return sjb200_stage1_sharded_delimited_finish(m, out);
+}
+
+// ---------------------------------------------------------------------------------------------- sharded stage-2-lite
+// Enqueue one tokens pass: the launches of sjb200_tokens_dev on the shard, on the totals and tile scratch of the pass's
+// own slot (passes of every kind may be in flight), with tile_scan_kernel storing the record and the summary into every
+// rank's window.  A rank that cannot run its pass (device allocation) still publishes a record, with kFlagInternal, so
+// that every rank's finish fails alike instead of waiting for it.
+extern "C" int sjb200_tokens_sharded_enqueue(sjb200_comm *m, const uint8_t *d_shard, size_t len, uint32_t state_in, const uint32_t *d_idx, uint32_t n,
+                                             uint8_t *d_type, uint64_t *d_payload, uint8_t *d_strbuf, size_t strbuf_capacity, void *stream) {
+  if (!m || !m->connected || len > kMaxBytes || state_in > 7u || (n && (!d_shard || !d_idx || !d_type || !d_payload)) || (strbuf_capacity && !d_strbuf))
+    return SJB200_UNEXPECTED_ERROR;
+  if (m->head - m->tail >= uint32_t(kXchgSteps / 2)) return SJB200_CAPACITY;  // too many passes in flight: finish some first
+  sjb200_ctx *c = m->ctx;
+  DeviceGuard g(c->device);
+  const auto t_enq = std::chrono::steady_clock::now();
+  cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : c->stream;
+  const uint32_t seq = m->head + 1, i = m->head % uint32_t(kXchgSteps);
+  sjb200_comm::Step &st = m->steps[i];
+  st.d_buf = d_shard; st.len = len; st.d_idx = nullptr; st.d_dst = nullptr; st.stream = s; st.seq = seq; st.last = 0; st.kind = kTokens; st.mode = 0;
+  TokXchg x{};
+  for (int r = 0; r < kMaxRanks; r++) x.peer[r] = m->peer[r];
+  x.nranks = uint32_t(m->nranks); x.rank = uint32_t(m->rank); x.slot = window_slot(seq, 0); x.seq = seq;
+  x.state_in = state_in; x.n = n; x.len = len; x.capacity = strbuf_capacity;
+  const size_t need = tokens_scratch_bytes(n);
+  bool have = m->d_tok_tot || dev_alloc(c, &m->d_tok_tot, kXchgSteps, "cudaMalloc(token totals)");
+  if (have && m->tok_scratch_bytes[i] < need) {  // (the slot's previous pass has been finished: at most kXchgSteps / 2 are in flight)
+    cudaFree(m->d_tok_scratch[i]); m->d_tok_scratch[i] = nullptr; m->tok_scratch_bytes[i] = 0;
+    have = ok(c, cudaMalloc(&m->d_tok_scratch[i], need), "cudaMalloc(token scratch)");
+    if (have) m->tok_scratch_bytes[i] = need;
+  }
+  bool good;
+  if (have) {
+    good = ok(c, launch_tokens(d_shard, len, d_idx, n, d_type, d_payload, d_strbuf, strbuf_capacity, m->d_tok_scratch[i], m->d_tok_tot + i,
+                               int(c->opt_tok_stage), s, &x), "tokens");
+    c->launches += good ? (n ? 3 : 1) : 0;
+  } else {
+    ScanParams p;
+    memset(&p, 0, sizeof(p));
+    for (int r = 0; r < kMaxRanks; r++) p.xchg_peer[r] = m->peer[r];
+    p.xchg_nranks = x.nranks; p.xchg_rank = x.rank; p.xchg_slot = x.slot; p.xchg_seq = seq;
+    good = ok(c, launch_xchg_post(p, xchg_word0(seq, 0), xchg_word1(seq, state_in, 0, kFlagInternal, kTokens), s), "xchg post");
+    c->launches += good ? 1 : 0;
+  }
+  if (!good || !ok(c, cudaEventRecord(m->done[i], s), "event record")) return SJB200_UNEXPECTED_ERROR;
+  m->head++;
+  c->xchg_enqueue_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_enq).count();
+  return SJB200_SUCCESS;
+}
+
+// Complete the oldest pass in flight, a tokens pass: the own pass's event, the records (round 0: kind, dirty cuts, short
+// and failed ranks), the summaries (round 2), then the fold of the bases and of the first error.  No second round: a
+// dirty cut is refused, not re-run.
+extern "C" int sjb200_tokens_sharded_finish(sjb200_comm *m, sjb200_sharded_tokens_result *out) {
+  if (!m || !out || m->tail == m->head) return SJB200_UNEXPECTED_ERROR;
+  sjb200_ctx *c = m->ctx;
+  DeviceGuard g(c->device);
+  memset(out, 0, sizeof(*out));
+  out->error = SJB200_UNEXPECTED_ERROR;
+  out->first_error_index = UINT64_MAX;
+  const uint32_t slot_i = m->tail % uint32_t(kXchgSteps);
+  const sjb200_comm::Step st = m->steps[slot_i];
+  if (st.kind != kTokens) {  // (the pass stays in flight: the caller can still finish it with the right call)
+    c->last_error = "sharded finish: the oldest pass in flight is of another kind";
+    return SJB200_UNEXPECTED_ERROR;
+  }
+  m->tail++;
+  const auto t_ev = std::chrono::steady_clock::now();
+  if (!ok(c, cudaEventSynchronize(m->done[slot_i]), "event sync")) return SJB200_UNEXPECTED_ERROR;  // own launches (and their stores) done
+  c->xchg_evsync_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_ev).count();
+  int rc = comm_collect(m, st.seq, 0);
+  if (rc != SJB200_SUCCESS) return rc;
+  int failed = -1;
+  for (int r = 0; r < m->nranks; r++) {
+    const unsigned long long w1 = m->h_rec[2 * r + 1];
+    if (xchg_kind(w1) != kTokens) {
+      c->last_error = "sharded pass " + std::to_string(st.seq) + ": rank " + std::to_string(r) + " published a pass of another kind (every rank must enqueue the same sequence of kinds)";
+      return SJB200_UNEXPECTED_ERROR;
+    }
+    const uint32_t fl = uint32_t(w1 >> 16) & 0xFFu;
+    if (w1 & 7u) out->dirty_cuts |= 1u << r;
+    if (fl & kTokShortFlag) out->short_ranks |= 1u << r;
+    if ((fl & kFlagInternal) && failed < 0) failed = r;
+  }
+  if (out->dirty_cuts) {
+    const int r = __builtin_ctz(out->dirty_cuts);
+    c->last_error = "sharded tokens pass " + std::to_string(st.seq) + ": rank " + std::to_string(r) + " starts in state " +
+                    std::to_string(m->h_rec[2 * r + 1] & 7u) + ", inside a token (tokens need cuts where the state is 0, e.g. after a line feed)";
+    return SJB200_UNEXPECTED_ERROR;
+  }
+  if (failed >= 0) {
+    if (failed != m->rank) c->last_error = "sharded tokens pass " + std::to_string(st.seq) + ": rank " + std::to_string(failed) + " could not run its pass";
+    return SJB200_UNEXPECTED_ERROR;
+  }
+  rc = comm_collect(m, st.seq, 2);
+  if (rc != SJB200_SUCCESS) return rc;
+  uint64_t tokens = 0, bytes = 0, strings = 0, string_bytes = 0;
+  int err = SJB200_SUCCESS;
+  for (int r = 0; r < m->nranks; r++) {
+    const unsigned long long *w = m->h_rec + size_t(r) * kSumWords;
+    const uint64_t sb = uint64_t(uint32_t(w[5])) | (uint64_t(uint32_t(w[6])) << 32);
+    const uint32_t code = uint32_t(w[4]) & 0xFFu;
+    if (err == SJB200_SUCCESS && code != 0) {  // the earliest rank's first token in error
+      err = int(code);
+      out->first_error_index = tokens + uint32_t(w[3]);
+    }
+    if (r == m->rank) {
+      out->tokens_before = tokens; out->bytes_before = bytes; out->strings_before = strings; out->string_base = string_bytes;
+      out->n_strings = uint32_t(w[2]); out->string_bytes = sb;
+    }
+    tokens += uint32_t(w[1]); bytes += uint32_t(w[0]); strings += uint32_t(w[2]); string_bytes += sb;
+  }
+  out->total_strings = strings;
+  out->total_string_bytes = string_bytes;
+  if (err == SJB200_SUCCESS && out->short_ranks) err = SJB200_CAPACITY;
+  out->error = err;
+  return err;
+}
+
+extern "C" int sjb200_tokens_sharded(sjb200_comm *m, const uint8_t *d_shard, size_t len, uint32_t state_in, const uint32_t *d_idx, uint32_t n,
+                                     uint8_t *d_type, uint64_t *d_payload, uint8_t *d_strbuf, size_t strbuf_capacity, sjb200_sharded_tokens_result *out,
+                                     void *stream) {
+  int rc = sjb200_tokens_sharded_enqueue(m, d_shard, len, state_in, d_idx, n, d_type, d_payload, d_strbuf, strbuf_capacity, stream);
+  if (rc != SJB200_SUCCESS) return rc;
+  return sjb200_tokens_sharded_finish(m, out);
 }
 
 // The fold of a delimited pass's filter round into the whole stream's finish() for modes 3..6 (json_structural_indexer.h

@@ -19,8 +19,12 @@ constexpr int kXchgSteps = 64;                        // sharded passes whose ex
 #endif
 
 // ---- scan kinds (kStream: a stage-1 pass of the sharded streaming modes; kDelim: one of the sharded RS / comma-delimited
-// modes.  Both scan like kIndex, only their records differ)
-enum : int { kIndex = 0, kMinify = 1, kUtf8 = 2, kStream = 3, kDelim = 4 };
+// modes.  Both scan like kIndex, only their records differ.  kTokens: a sharded stage-2-lite pass, whose record comes
+// from tile_scan_kernel, sjb200_tape.cu)
+enum : int { kIndex = 0, kMinify = 1, kUtf8 = 2, kStream = 3, kDelim = 4, kTokens = 5 };
+// a kTokens record's flags: kFlagInternal (the rank could not run its pass), or this rank's string bytes exceed its
+// string buffer (it wrote no records)
+constexpr uint32_t kTokShortFlag = 8u;
 
 // Scanner state between consecutive launches of one document (chunked streaming,
 // multi-GPU shards).  state: bit0 escape, bit1 in_string, bit2 prev_scalar.
@@ -98,9 +102,10 @@ struct ScanParams {
 #endif
 // one shard record as two independently tagged 64-bit words (8-byte stores are single transactions):
 //   w0 = seq[30:0] << 33 | count[32:0]        w1 = seq << 32 | kind << 24 | flags << 16 | ttable << 8 | state_out
-// kind (3 bits, 24-26) is the scan kind of the pass (kIndex 0, kMinify 1, kUtf8 2, kStream 3, kDelim 4); count is
-// structurals (kIndex, kStream, kDelim), kept bytes (kMinify) or 0 (kUtf8).  Bit 26 was zero before kDelim existed, so the
-// records of the other kinds are unchanged.
+// kind (3 bits, 24-26) is the scan kind of the pass (kIndex 0, kMinify 1, kUtf8 2, kStream 3, kDelim 4, kTokens 5); count
+// is structurals (kIndex, kStream, kDelim), kept bytes (kMinify), 0 (kUtf8) or string bytes (kTokens, whose state_out
+// field carries the state the caller says the shard starts in).  Bit 26 was zero before kDelim existed, so the records of
+// the other kinds are unchanged.
 SJ_PARAMS_HD inline unsigned long long xchg_word0(uint32_t seq, uint64_t count) {
   return ((unsigned long long)(seq & 0x7FFFFFFFu) << 33) | (count & 0x1FFFFFFFFull);
 }
@@ -122,6 +127,9 @@ SJ_PARAMS_HD inline uint64_t xchg_count(unsigned long long w0) { return w0 & 0x1
 //   start on, or over every kept structural when there is none
 //   7 role of the first kept structural | role of the last << 3 | has an internal start << 6   (roles: kRole*, sjb200_docs.cu)
 // (whether byte 0 is a structural is word 1 == 0 with a count > 0; the counts come from the records)
+// A tokens pass (kTokens) stores its summary in the same place, from tile_scan_kernel:
+//   0 shard length   1 n (tokens)   2 strings   3 local index of the first token in error (0xFFFFFFFF: none)   4 its
+//   error code (0: none)   5 / 6 low / high 32 bits of the string bytes   7 zero
 constexpr int kSumWords = 8;
 constexpr size_t kXchgRecordWords = size_t(kXchgSteps) * 2 * kMaxRanks * 2;
 constexpr size_t kXchgSummaryWords = size_t(kXchgSteps) * kMaxRanks * kSumWords;

@@ -15,7 +15,8 @@
 // Three launches, no host round trip between them; a tile = kTokThreads consecutive structurals, one per thread:
 //   A  token_scan_kernel   type and payload of every token (a string's payload is its unescaped length for now),
 //                          per-tile sums of the string_buf bytes
-//   S  tile_scan_kernel    exclusive scan of the tile sums (one CTA), totals
+//   S  tile_scan_kernel    exclusive scan of the tile sums (one CTA), totals; in a sharded pass (sjb200_comm) also the
+//                          shard's record and summary, stored into every rank's exchange window
 //   B  string_write_kernel every string's record offset (tile offset + CTA scan), the record itself (second walk over
 //                          the string, now writing), payload = offset
 // Data movement: the bytes a tile's tokens live in are one contiguous span of the document (from its first structural to
@@ -139,8 +140,11 @@ __global__ void __launch_bounds__(kTokThreads) token_scan_kernel(const uint8_t *
   }
 }
 
-// ---- S: exclusive scan of tile_bytes in place (one CTA), totals
-__global__ void __launch_bounds__(1024) tile_scan_kernel(unsigned long long *tile_bytes, const uint32_t *tile_strings, uint32_t ntiles, TokenTotals *tot) {
+// ---- S: exclusive scan of tile_bytes in place (one CTA), totals.  In a sharded pass it also publishes the shard's record
+// and summary (sjb200_params.h) into every rank's window: everything they carry is known here -- A's atomicMin have all
+// landed (A ran before S on the stream), the totals are this kernel's.  It stores and leaves; nothing waits for a peer.
+__global__ void __launch_bounds__(1024) tile_scan_kernel(unsigned long long *tile_bytes, const uint32_t *tile_strings, uint32_t ntiles, TokenTotals *tot,
+                                                         TokXchg x) {
   __shared__ unsigned long long sh[32];
   __shared__ unsigned long long carry;
   __shared__ uint32_t shs[32];
@@ -181,6 +185,25 @@ __global__ void __launch_bounds__(1024) tile_scan_kernel(unsigned long long *til
     for (int w = 0; w < 32; w++) s += shs[w];
     tot->n_strings = s;
     tot->string_bytes = carry;
+    if (x.nranks != 0) {
+      const unsigned long long fe = tot->first_error;
+      const uint32_t w[kSumWords] = {uint32_t(x.len), x.n, s, fe == ~0ull ? 0xFFFFFFFFu : uint32_t(fe >> 8), fe == ~0ull ? 0u : uint32_t(fe & 0xFFull),
+                                     uint32_t(carry), uint32_t(carry >> 32), 0u};
+      const unsigned long long w0 = xchg_word0(x.seq, carry),
+                               w1 = xchg_word1(x.seq, x.state_in, 0, carry > x.capacity ? kTokShortFlag : 0u, kTokens);
+#pragma unroll
+      for (uint32_t r = 0; r < uint32_t(kMaxRanks); r++) {  // (unrolled: x.peer stays in the parameter space, no stack copy)
+        if (r >= x.nranks) break;
+        unsigned long long *sum = x.peer[r] + xchg_summary_at(x.seq, x.rank);
+        for (int k = 0; k < kSumWords; k++) {
+          const unsigned long long v = (static_cast<unsigned long long>(x.seq) << 32) | w[k];
+          asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(sum + k), "l"(v) : "memory");
+        }
+        unsigned long long *rec = x.peer[r] + (size_t(x.slot) * kMaxRanks + x.rank) * 2;
+        asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(rec), "l"(w0) : "memory");
+        asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(rec + 1), "l"(w1) : "memory");
+      }
+    }
   }
 }
 
@@ -272,19 +295,21 @@ size_t tokens_scratch_bytes(uint32_t n) {
 }
 
 cudaError_t launch_tokens(const uint8_t *buf, uint64_t len, const uint32_t *idx, uint32_t n, uint8_t *type, uint64_t *payload, uint8_t *strbuf,
-                          uint64_t strbuf_capacity, void *scratch, TokenTotals *tot_dev, int stage, cudaStream_t stream) {
+                          uint64_t strbuf_capacity, void *scratch, TokenTotals *tot_dev, int stage, cudaStream_t stream, const TokXchg *xchg) {
   const uint32_t tiles = uint32_t((size_t(n) + kTokThreads - 1) / kTokThreads);
   unsigned long long *tile_bytes = static_cast<unsigned long long *>(scratch);
   uint32_t *tile_strings = reinterpret_cast<uint32_t *>(tile_bytes + tiles);
+  TokXchg x{};
+  if (xchg) x = *xchg;
   cudaError_t e = cudaMemsetAsync(tot_dev, 0xFF, sizeof(TokenTotals), stream);  // first_error = ~0; the scan kernel stores the other fields
   if (e != cudaSuccess) return e;
   if (n == 0) {
-    tile_scan_kernel<<<1, 1024, 0, stream>>>(tile_bytes, tile_strings, 0, tot_dev);
+    tile_scan_kernel<<<1, 1024, 0, stream>>>(tile_bytes, tile_strings, 0, tot_dev, x);
     return cudaGetLastError();
   }
   token_scan_kernel<<<tiles, kTokThreads, 0, stream>>>(buf, len, idx, n, type, reinterpret_cast<unsigned long long *>(payload), tile_bytes, tile_strings, tot_dev,
                                                        stage);
-  tile_scan_kernel<<<1, 1024, 0, stream>>>(tile_bytes, tile_strings, tiles, tot_dev);
+  tile_scan_kernel<<<1, 1024, 0, stream>>>(tile_bytes, tile_strings, tiles, tot_dev, x);
   string_write_kernel<<<tiles, kTokThreads, 0, stream>>>(buf, len, idx, n, type, reinterpret_cast<unsigned long long *>(payload), tile_bytes, tiles, strbuf,
                                                          strbuf_capacity, tot_dev, stage);
   return cudaGetLastError();

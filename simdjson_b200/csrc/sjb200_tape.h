@@ -4,6 +4,8 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include "sjb200_params.h"
+
 namespace sjb200 {
 
 struct TokenTotals {
@@ -13,11 +15,24 @@ struct TokenTotals {
   uint32_t reserved;
 };
 
+// A sharded tokens pass (sjb200_comm): where tile_scan_kernel stores the shard's record (window slot `slot`, kind
+// kTokens) and its summary (xchg_summary_at(seq, rank)) in every rank's window, and what they carry besides the totals.
+// nranks == 0: no exchange.
+struct TokXchg {
+  unsigned long long *peer[kMaxRanks];
+  uint32_t nranks, rank, slot, seq;
+  uint32_t state_in;   // the scanner state the caller says the shard starts in (0: a clean cut)
+  uint32_t n;
+  uint64_t len;
+  uint64_t capacity;   // this rank's string buffer
+};
+
 size_t tokens_scratch_bytes(uint32_t n);
 // type[n], payload[n], strbuf[strbuf_capacity]: device memory; scratch: tokens_scratch_bytes(n) bytes, 8-byte aligned;
 // stage: 1 = tiles staged through shared memory (the product path), 0 = every thread reads / writes global memory (kept as
-// the A/B baseline of the staging, option tok_stage)
+// the A/B baseline of the staging, option tok_stage).  xchg: a sharded pass's exchange, fused into the scan of the tile
+// sums (null: none)
 cudaError_t launch_tokens(const uint8_t *buf, uint64_t len, const uint32_t *idx, uint32_t n, uint8_t *type, uint64_t *payload, uint8_t *strbuf,
-                          uint64_t strbuf_capacity, void *scratch, TokenTotals *tot_dev, int stage, cudaStream_t stream);
+                          uint64_t strbuf_capacity, void *scratch, TokenTotals *tot_dev, int stage, cudaStream_t stream, const TokXchg *xchg = nullptr);
 
 }  // namespace sjb200

@@ -1,6 +1,6 @@
 """Multi-GPU sharding of one stage-1 scan (SURVEY.md section 8e): the host-side protocol around
-`sjb200_stage1_shard_dev`, and `Comm`, the per-rank object of the sharded stage-1 / minify / validate_utf8 passes whose
-exchange is fused into the kernels.
+`sjb200_stage1_shard_dev`, and `Comm`, the per-rank object of the sharded stage-1 / minify / validate_utf8 / stage-2-lite
+passes whose exchange is fused into the kernels.
 
 Every rank scans its byte range with a *speculated* incoming scanner state (0 = outside a string, no pending
 escape, previous byte not a scalar).  A shard's 6-bit carry transducer does not depend on the incoming state, so
@@ -9,6 +9,7 @@ whose speculation was wrong scans again with the true state and a second all-gat
 Indexes stay shard-relative (uint32) plus a 64-bit base, like document_stream's batch_start + structural_indexes[i]
 (include/simdjson/dom/document_stream-inl.h L250).
 """
+import collections
 import ctypes as C
 
 import numpy as np
@@ -98,6 +99,7 @@ class Comm:
         from . import capi
         self._capi = capi
         self.parser, self.rank, self.world = parser, rank, world
+        self._tokens_out = collections.deque()  # the outputs of the tokens passes in flight, oldest first
         self._h = C.c_void_p()
         rc = _lib().sjb200_comm_create(parser._ctx, rank, world, C.byref(self._h))
         if rc != 0:
@@ -218,6 +220,44 @@ class Comm:
         if rc != 0:
             return rc, None
         return self.delimited_finish()
+
+    # stage-2-lite over this shard's structurals; its passes share the window with the other kinds
+    def tokens_enqueue(self, d_shard, d_idx, n, state_in, strbuf_capacity=None, stream=None):
+        """(d_idx, n): this shard's structurals from a sharded stage-1 pass (count, or kept for a stream / delimited pass),
+        state_in: that pass's folded state_in (it must be 0).  Allocates the outputs the way
+        dom_parser_implementation.tokens_device does (string buffer: sjb200_string_buf_capacity(len(shard)) bytes by
+        default) and keeps them until tokens_finish returns them."""
+        import torch
+
+        from .implementation import _stream_ptr
+        n = int(n)
+        cap = int(_lib().sjb200_string_buf_capacity(d_shard.numel())) if strbuf_capacity is None else int(strbuf_capacity)
+        dev = d_shard.device
+        d_type = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)
+        d_payload = torch.empty(max(n, 1), dtype=torch.int64, device=dev)
+        d_strbuf = torch.empty(max(cap, 1), dtype=torch.uint8, device=dev)
+        rc = _lib().sjb200_tokens_sharded_enqueue(self._h, d_shard.data_ptr(), d_shard.numel(), int(state_in), d_idx.data_ptr(), n, d_type.data_ptr(),
+                                                  d_payload.data_ptr(), d_strbuf.data_ptr() if cap else None, cap, _stream_ptr(stream))
+        if rc == 0:
+            self._tokens_out.append((d_type[:n], d_payload[:n], d_strbuf))
+        return rc
+
+    def tokens_finish(self):
+        """(error_code, ShardedTokensResult, d_type uint8[n], d_payload int64[n] (bit pattern of the uint64), d_strbuf) of
+        the oldest pass in flight.  Outputs are shard-relative: '"' payloads + string_base and 'd' payloads + bytes_before
+        are the whole document's; d_strbuf[:string_bytes] is this rank's part of its string buffer."""
+        res = self._capi.ShardedTokensResult()
+        rc = _lib().sjb200_tokens_sharded_finish(self._h, C.byref(res))
+        if rc == self._capi.UNEXPECTED_ERROR and "oldest pass in flight is of another kind" in self.parser.last_cuda_error():
+            return rc, res, None, None, None  # (it stays in flight, and so do the outputs of the tokens passes)
+        d_type, d_payload, d_strbuf = self._tokens_out.popleft() if self._tokens_out else (None, None, None)
+        return rc, res, d_type, d_payload, d_strbuf
+
+    def tokens(self, d_shard, d_idx, n, state_in, strbuf_capacity=None, stream=None):
+        rc = self.tokens_enqueue(d_shard, d_idx, n, state_in, strbuf_capacity, stream)
+        if rc != 0:
+            return rc, None, None, None, None
+        return self.tokens_finish()
 
     def document_table(self, d_shard, d_idx, result, stream=None):
         """the document starts among this shard's kept structurals (result: a ShardedStreamResult, or the `stream` field of
