@@ -19,6 +19,8 @@
 #include <thread>
 #include <vector>
 
+#include "simt_fenced.h"
+
 extern "C" {
 #include "sj_oracle.h"
 }
@@ -108,12 +110,13 @@ struct Result {
 };
 
 // one document (or shard) through 1..n launches of chunk_tiles tiles each, like scan_host_document
+// (idx_ext: the index output goes there instead of into Result::idx)
 Result run_scan4(EmuCtx &cx, const uint8_t *buf, size_t len, uint32_t state_in, uint32_t chunk_tiles, unsigned grid, bool use_tma,
-                 bool sentinels, uint8_t *minify_dst = nullptr) {
+                 bool sentinels, uint8_t *minify_dst = nullptr, uint32_t *idx_ext = nullptr) {
   Result r;
   const uint32_t ntiles_total = uint32_t((len + kTileBytes - 1) / kTileBytes);
   if (cx.desc.size() < size_t(ntiles_total) + 1) cx.desc.assign(size_t(ntiles_total) + 1, 0ull);
-  r.idx.assign(len + 80, 0xABABABABu);
+  if (!idx_ext) r.idx.assign(len + 80, 0xABABABABu);
   sj_tensor_map tmap;
   tmap.base = buf;
   tmap.rows = len / 128;
@@ -132,7 +135,7 @@ Result run_scan4(EmuCtx &cx, const uint8_t *buf, size_t len, uint32_t state_in, 
     p.use_tma = tma_ok ? 1u : 0u;
     p.tile_begin = tb; p.ntiles = nt;
     p.epoch = ++cx.epoch;
-    p.idx_out = r.idx.data(); p.dst = minify_dst;
+    p.idx_out = idx_ext ? idx_ext : r.idx.data(); p.dst = minify_dst;
     p.write_sentinels = (sentinels && !minify_dst && tb + nt == ntiles_total) ? 1u : 0u;
     p.carry_in = &cx.carry[slot];
     p.carry_out = &cx.carry[slot + 1];
@@ -322,9 +325,7 @@ int check_minify(EmuCtx &cx, const std::vector<uint8_t> &store, size_t misalign,
 }
 
 // validate_utf8 with independent warps (sjb200_utf8.cuh) against the oracle; chunk_tiles > 0: several launches like the host path
-int check_utf8v2(EmuCtx &cx, const std::vector<uint8_t> &store, size_t misalign, uint32_t chunk_tiles, unsigned grid, bool use_tma) {
-  const uint8_t *buf = store.data() + misalign;
-  const size_t len = store.size() - misalign;
+int check_utf8v2(EmuCtx &cx, const uint8_t *buf, size_t len, size_t misalign, uint32_t chunk_tiles, unsigned grid, bool use_tma) {
   if (len == 0) return 0;
   const uint32_t ntiles_total = uint32_t((len + kTileBytes - 1) / kTileBytes);
   sj_tensor_map tmap;
@@ -357,10 +358,124 @@ int check_utf8v2(EmuCtx &cx, const std::vector<uint8_t> &store, size_t misalign,
   }
   return 0;
 }
+int check_utf8v2(EmuCtx &cx, const std::vector<uint8_t> &store, size_t misalign, uint32_t chunk_tiles, unsigned grid, bool use_tma) {
+  return check_utf8v2(cx, store.data() + misalign, store.size() - misalign, misalign, chunk_tiles, grid, use_tma);
+}
+
+// ---- fenced pass: every buffer the kernels are given is exactly as long as the C API promises and sits right against a
+// PROT_NONE page, so a read of the input or a write of an output outside its bounds kills the process instead of going
+// unnoticed (the TMA full-block predicate, the guarded fill of the last block, the look-backs before byte 0, the 16-byte
+// copy-outs of the stage-1 and minify emits, the sentinel words)
+// (Fenced, index_words: simt_fenced.h)
+
+// a document that changes its result if one byte more is read at either end: it starts with a continuation byte, a quote,
+// a backslash or a digit and ends in a backslash, an open string, a partial or complete UTF-8 character, a number or a
+// truncated atom; backslash runs and quotes sit on the block boundaries in between
+std::vector<uint8_t> fenced_doc(std::mt19937_64 &rng, size_t len) {
+  static const char *alpha = "\\\\\\\"\" {}[],: \n\tabc1\x01\x1e";
+  static const char *heads[] = {"\x80", "\"", "\\", "7"};
+  static const char *tails[] = {"\\", "\"ab", "\xf0\x9f\x98", "\xe2\x82\xac", "123", "tru", "\xc3"};
+  std::vector<uint8_t> d(len);
+  const size_t alen = strlen(alpha);
+  for (size_t i = 0; i < len; i++) d[i] = uint8_t(rng() % 3 ? alpha[rng() % alen] : 'a' + rng() % 26);
+  for (size_t b = 128; b + 8 < len; b += 128)
+    if (b % 4096 == 0 || rng() % 8 == 0) {
+      const size_t run = 1 + rng() % 5;
+      for (size_t k = 0; k < run && b - k > 0; k++) d[b - k] = '\\';
+      if (rng() % 2) d[b + 1] = '"';
+    }
+  if (len == 0) return d;
+  const char *h = heads[rng() % 4];
+  d[0] = uint8_t(h[0]);
+  const char *t = tails[rng() % 7];
+  const size_t tl = std::min(strlen(t), len);
+  memcpy(d.data() + len - tl, t + strlen(t) - tl, tl);
+  return d;
+}
+
+int fenced_case(EmuCtx &cx, const std::vector<uint8_t> &doc, bool in_at_end, bool out_at_end, bool use_tma, uint32_t state_in, bool sentinels, unsigned grid,
+                bool minify, bool utf8) {
+  const size_t len = doc.size();
+  Fenced in(len, in_at_end);
+  memcpy(in.p, doc.data(), len);
+  const uint8_t *buf = in.p;
+  int bad = 0;
+  {  // stage 1 (sentinels) / a shard that is not the last (sjb200_stage1_shard_dev: none): exactly sjb200_index_words(len) words
+    const size_t words = index_words(len);
+    Fenced out(words * 4, out_at_end);
+    uint32_t *idx = reinterpret_cast<uint32_t *>(out.p);
+    for (size_t i = 0; i < words; i++) idx[i] = 0xABABABABu;
+    Result r = run_scan4(cx, buf, len, state_in, 0, grid, use_tma, sentinels, nullptr, idx);
+    std::vector<uint32_t> oidx(len + 16);
+    uint32_t ostate = 0;
+    const uint64_t on = sjo_scan_shard(buf, len, state_in, oidx.data(), &ostate);
+    if (r.flags & kFlagInternal) bad = 1;
+    else if (r.count != on || memcmp(idx, oidx.data(), on * 4) != 0) bad = 2;
+    else if (sentinels && (idx[on] != uint32_t(len) || idx[on + 1] != uint32_t(len) || idx[on + 2] != 0)) bad = 3;
+    else if (r.state != (ostate & 7u) || r.ttable != sjo_transducer(buf, len)) bad = 4;
+    else if (bool(r.flags & kFlagUtf8) == bool(sjo_validate_utf8(buf, len))) bad = 5;
+    for (size_t i = on + (sentinels ? 3 : 0); i < words && !bad; i++)
+      if (idx[i] != 0xABABABABu) bad = 6;  // a word past the structurals (and sentinels)
+  }
+  if (!bad && minify) {  // minify: dst exactly len bytes
+    Fenced out(len, out_at_end);
+    memset(out.p, 0xEE, len);
+    Result r = run_scan4(cx, buf, len, 0, 0, grid, use_tma, false, out.p);
+    std::vector<uint8_t> want(len + 1);
+    size_t wlen = 0;
+    const int werr = sjo_minify(buf, len, want.data(), &wlen);
+    const bool unclosed = (r.state >> 1) & 1u;
+    if (r.flags & kFlagInternal) bad = 11;
+    else if (unclosed != (werr == SJO_UNCLOSED_STRING)) bad = 12;
+    else if (!unclosed && (r.count != wlen || memcmp(out.p, want.data(), wlen) != 0)) bad = 13;
+    for (size_t i = size_t(r.count); i < len && !bad; i++)
+      if (out.p[i] != 0xEE) bad = 14;
+  }
+  if (bad) {
+    fprintf(stderr, "FENCED MISMATCH kind=%d len=%zu in_at_end=%d out_at_end=%d tma=%d state_in=%u sentinels=%d grid=%u\n", bad, len, int(in_at_end),
+            int(out_at_end), int(use_tma), state_in, int(sentinels), grid);
+    hexdump(doc);
+    g_fail++;
+  }
+  if (!bad && utf8) bad = check_utf8v2(cx, buf, len, 0, 0, grid, use_tma);
+  return bad;
+}
+
+int run_fenced(std::mt19937_64 &rng) {
+  EmuCtx cx;
+  const size_t T = kTileBytes;
+  const size_t lens[] = {1, 3, 4, 5, 16, 127, 128, 129, 4095, 4096, 4097, 8192 + 127, 8192 + 128, T - 1, T, T + 1, 2 * T + 128, 3 * T + 4095};
+  int cases = 0;
+  for (size_t len : lens) {
+    for (int placement = 0; placement < 4; placement++) {
+      const bool in_at_end = (placement & 1) == 0, out_at_end = (placement & 2) == 0;
+      for (int tma = 1; tma >= 0; tma--) {
+        const std::vector<uint8_t> doc = fenced_doc(rng, len);
+        const unsigned grid = 1 + unsigned(rng() % 2);
+        // every incoming shard state on the short documents, one random state on the long ones
+        const uint32_t nstates = len <= 4097 && placement == 0 ? 8u : 1u;
+        for (uint32_t s = 0; s < nstates; s++) {
+          const uint32_t state_in = nstates == 8 ? s : uint32_t(rng() % 8);
+          fenced_case(cx, doc, in_at_end, out_at_end, tma != 0, state_in, (cases & 1) == 0, grid, s == 0, s == 0);
+          cases++;
+          if (g_fail >= 5) return g_fail;
+        }
+      }
+    }
+  }
+  printf("fenced pass: %d cases\n", cases);
+  return g_fail;
+}
 
 }  // namespace
 
 int main(int argc, char **argv) {
+  if (argc > 1 && strcmp(argv[1], "--fenced") == 0) {
+    std::mt19937_64 frng(0xfe9ced);
+    if (run_fenced(frng)) { printf("FAILED\n"); return 1; }
+    printf("simt emulation, fenced buffers OK\n");
+    return 0;
+  }
   const int iters = argc > 1 ? atoi(argv[1]) : 120;
   std::mt19937_64 rng(0x5eed1234);
   const char *alphabets[] = {"\\\\\\\"\" {}[],: \n\tabc1\x01\x0c\x1a\x1e", "\\\"", "\\\\\\\\\\\\\\\"a ", "\"{}[],:0 ", " \n\r\t\"a\\", ",{}[] 1 \"a\":\n"};

@@ -14,6 +14,8 @@
 #include <random>
 #include <vector>
 
+#include "simt_fenced.h"
+
 extern "C" {
 #include "sj_oracle.h"
 }
@@ -85,29 +87,54 @@ std::vector<uint8_t> random_doc(std::mt19937_64 &rng) {
 
 int g_fail = 0;
 
-// one launch over `docs`; misalign[k] != 0: the document starts that many bytes past a 16-byte boundary (plain loads)
-void check_launch(std::vector<std::vector<uint8_t>> &docs, const std::vector<size_t> &misalign, unsigned grid, uint32_t epoch, const char *what) {
+// one launch over `docs`; misalign[k] != 0: the document starts that many bytes past a 16-byte boundary (plain loads).
+// packed: the documents are consecutive, gapless pieces of one buffer (NDJSON rows in memory: a neighbour ends in a
+// backslash, inside a string, on a UTF-8 lead byte), and their index arrays are consecutive pieces of exactly
+// sjb200_index_words(len) words of another; both buffers end at an inaccessible page (the input starts right after one
+// when in_at_end is false), so a read outside the documents or a write outside the index arrays kills the process, and
+// the words of each array past its structurals and sentinels must still hold their fill
+void check_launch(std::vector<std::vector<uint8_t>> &docs, const std::vector<size_t> &misalign, unsigned grid, uint32_t epoch, const char *what,
+                  bool packed = false, bool in_at_end = true) {
   const size_t n = docs.size();
   std::vector<std::vector<uint8_t>> store(n);
   std::vector<std::vector<uint32_t>> idx(n);
+  std::vector<uint32_t *> ip(n);
+  std::vector<size_t> nwords(n);
+  size_t in_bytes = 0, out_words = 0;
+  for (size_t k = 0; k < n; k++) in_bytes += docs[k].size(), out_words += index_words(docs[k].size());
+  Fenced in(packed ? in_bytes : 0, in_at_end), out(packed ? out_words * 4 : 0, true);
+  size_t in_off = 0, out_off = 0;
   std::vector<sj_tensor_map> maps(n);
   std::vector<DocEntry> tab(n);
   std::vector<Carry> carry(n);
   std::vector<uint32_t> flags(n + 1, 0);
   uint32_t elems = 0;
   for (size_t k = 0; k < n; k++) {
-    store[k].assign(docs[k].size() + misalign[k] + 16, 0);
-    memcpy(store[k].data() + misalign[k], docs[k].data(), docs[k].size());
-    const uint8_t *buf = store[k].data() + misalign[k];
-    idx[k].assign(docs[k].size() + 16, 0xABABABABu);
+    const uint8_t *buf;
+    if (packed) {
+      memcpy(in.p + in_off, docs[k].data(), docs[k].size());
+      buf = in.p + in_off;
+      in_off += docs[k].size();
+      nwords[k] = index_words(docs[k].size());
+      ip[k] = reinterpret_cast<uint32_t *>(out.p) + out_off;
+      out_off += nwords[k];
+      for (size_t i = 0; i < nwords[k]; i++) ip[k][i] = 0xABABABABu;
+    } else {
+      store[k].assign(docs[k].size() + misalign[k] + 16, 0);
+      memcpy(store[k].data() + misalign[k], docs[k].data(), docs[k].size());
+      buf = store[k].data() + misalign[k];
+      idx[k].assign(docs[k].size() + 16, 0xABABABABu);
+      ip[k] = idx[k].data();
+      nwords[k] = idx[k].size();
+    }
     maps[k].base = buf; maps[k].rows = docs[k].size() / 128; maps[k].box_rows = scan4::kBlockRows;
     DocEntry &e = tab[k];
     e.buf = buf;
-    e.idx_out = idx[k].data();
+    e.idx_out = ip[k];
     e.carry_out = &carry[k];
     e.carry_out_host = nullptr;
     e.flags = &flags[1 + k];
-    e.tmap = (misalign[k] == 0 && maps[k].rows > 0) ? &maps[k] : nullptr;
+    e.tmap = (misalign[k] == 0 && (reinterpret_cast<uintptr_t>(buf) & 15u) == 0 && maps[k].rows > 0) ? &maps[k] : nullptr;
     e.len = uint32_t(docs[k].size());
     e.scan_end = e.len;
     e.first_elem = elems;
@@ -134,14 +161,16 @@ void check_launch(std::vector<std::vector<uint8_t>> &docs, const std::vector<siz
     int bad = 0;
     if (r.flags & kFlagInternal) bad = 1;
     else if (r.count != on) bad = 2;
-    else if (memcmp(idx[k].data(), oidx.data(), on * 4) != 0) bad = 3;
-    else if (idx[k][on] != uint32_t(len) || idx[k][on + 1] != uint32_t(len) || idx[k][on + 2] != 0) bad = 4;
+    else if (memcmp(ip[k], oidx.data(), on * 4) != 0) bad = 3;
+    else if (ip[k][on] != uint32_t(len) || ip[k][on + 1] != uint32_t(len) || ip[k][on + 2] != 0) bad = 4;
     else if ((r.state & 7u) != (ostate & 7u)) bad = 5;
     else if (bool(r.flags & kFlagUtf8) == bool(sjo_validate_utf8(buf, len))) bad = 6;
     else if (r.ttable != sjo_transducer(buf, len)) bad = 7;
+    for (size_t i = on + 3; i < nwords[k] && !bad; i++)
+      if (ip[k][i] != 0xABABABABu) bad = 8;  // a word past the structurals and sentinels
     if (bad) {
-      fprintf(stderr, "MISMATCH kind=%d (%s) doc %zu of %zu len=%zu misalign=%zu grid=%u: got n=%llu state=%u flags=%u | want n=%llu state=%u\n", bad, what, k, n, len,
-              misalign[k], grid, (unsigned long long)r.count, r.state, r.flags, (unsigned long long)on, ostate);
+      fprintf(stderr, "MISMATCH kind=%d (%s) doc %zu of %zu len=%zu misalign=%zu packed=%d grid=%u: got n=%llu state=%u flags=%u | want n=%llu state=%u\n", bad, what, k,
+              n, len, misalign[k], int(packed), grid, (unsigned long long)r.count, r.state, r.flags, (unsigned long long)on, ostate);
       g_fail++;
     }
   }
@@ -149,10 +178,35 @@ void check_launch(std::vector<std::vector<uint8_t>> &docs, const std::vector<siz
 
 }  // namespace
 
+// the packed, fenced launches: documents whose ends are hostile to a neighbour that reads across them
+int run_fenced(std::mt19937_64 &rng, uint32_t &epoch) {
+  static const char *tails[] = {"\\", "\"ab", "\xf0\x9f\x98", "\xc3", "12", "tru", "\\\\\\"};
+  static const char heads[] = {'\x80', '"', '\\', '7'};
+  for (int it = 0; it < 24 && g_fail < 5; it++) {
+    const size_t n = 2 + rng() % 7;
+    std::vector<std::vector<uint8_t>> docs;
+    for (size_t k = 0; k < n; k++) {
+      std::vector<uint8_t> d = random_doc(rng);
+      d[0] = uint8_t(heads[rng() % 4]);
+      const char *t = tails[rng() % 7];
+      const size_t tl = std::min(strlen(t), d.size());
+      memcpy(d.data() + d.size() - tl, t + strlen(t) - tl, tl);
+      docs.push_back(d);
+    }
+    check_launch(docs, std::vector<size_t>(n, 0), 1 + unsigned(rng() % 3), ++epoch, "packed, fenced", true, it % 2 == 0);
+  }
+  return g_fail;
+}
+
 int main(int argc, char **argv) {
-  const int iters = argc > 1 ? atoi(argv[1]) : 24;
   std::mt19937_64 rng(0xD0C5);
   uint32_t epoch = 0;
+  if (argc > 1 && strcmp(argv[1], "--fenced") == 0) {
+    if (run_fenced(rng, epoch)) { printf("FAILED\n"); return 1; }
+    printf("simt emulation of packed, fenced multi-document launches OK\n");
+    return 0;
+  }
+  const int iters = argc > 1 ? atoi(argv[1]) : 24;
   // a document that ends inside a string, then a multi-element one: the later elements' look-back windows reach across
   // the boundary into descriptors of the same epoch
   {
