@@ -85,7 +85,6 @@ SJB200_API int sjb200_device(const sjb200_ctx *ctx);
 /* last CUDA error string seen by this context ("" if none); for diagnostics only */
 SJB200_API const char *sjb200_last_cuda_error(const sjb200_ctx *ctx);
 /* tuning knobs, mostly for tests and bench: "use_tma" (0/1), "grid" (CTAs, 0 = auto), "chunk_bytes", "copy_threads",
- * "ew_min_bytes" (stage-1 launches of at least this size use the emit-warp build of the kernel; 0 = never),
  * "time_kernel" (0/1: record CUDA events around the scan kernel on its launch stream), "pdl" (0/1, default 1: the
  * scan launches of one sjb200_stage1_dev_batch call after the first may start while the previous one still runs),
  * "launch_stamps" (0/1: sjb200_get_launch_stamps); none changes results */
@@ -94,7 +93,6 @@ SJB200_API int sjb200_set_option(sjb200_ctx *ctx, const char *key, long value);
  * both per document: a launch that scans several documents (sjb200_stage1_dev_batch) counts its duration divided by
  * their number, and a sjb200_stage1_dev_batch call counts the span from its first scan launch to the end of its last
  * one (launches may overlap), divided by its documents; "launches" (kernels launched by this context so far),
- * "ew_launches" (of which on the emit-warp build),
  * "grid_index", "sm_count"; negative when unavailable */
 SJB200_API double sjb200_get_stat(sjb200_ctx *ctx, const char *key);
 

@@ -35,7 +35,6 @@ constexpr int kTmapCacheEntries = 64;
 struct TmapCacheEntry {
   const uint8_t *base = nullptr;
   uint64_t rows = 0;
-  int box_rows = 0;
   CUtensorMap map;
 };
 constexpr size_t kMaxBytes = 0xFFFFFFFFull;  // SIMDJSON_MAXSIZE_BYTES (include/simdjson/base.h L23)
@@ -77,7 +76,6 @@ struct sjb200_ctx {
   StreamFinish *d_sfin = nullptr;  // [kCarrySlots] results of the device-side streaming epilogue
   uint32_t *d_doc_scratch = nullptr; size_t doc_scratch_words = 0; uint32_t *d_ndocs = nullptr;
   void *d_tok_scratch = nullptr; size_t tok_scratch_bytes = 0; TokenTotals *d_tok_tot = nullptr;  // stage-2-lite (sjb200_tape.cu)
-  uint32_t *d_park = nullptr; size_t d_park_words = 0;  // scan4 with emit warps: parked masks (a per-CTA ring, independent of the input size)
   int grid_u = 0;
   // pinned host mirrors
   Carry *h_carry = nullptr;     // [kCarrySlots]
@@ -102,7 +100,6 @@ struct sjb200_ctx {
   long opt_pdl = 1, opt_launch_stamps = 0;
   unsigned long long *d_debug = nullptr; size_t debug_tiles = 0; uint32_t debug_last_tiles = 0;
   unsigned long long launches = 0;               // kernels of ours launched by this context
-  unsigned long long ew_launches = 0;            // ... of which stage-1 launches on the emit-warp build
   PFN_encodeTiled encode = nullptr;
   TmapCacheEntry tmap_cache[kTmapCacheEntries];  // make_tensor_map
   // host-pointer pipeline: ring of page-locked staging slots filled by copy threads (sjb200_hostpipe.h)
@@ -110,8 +107,6 @@ struct sjb200_ctx {
   std::vector<cudaEvent_t> ring_events;
   CopyPool *pool = nullptr;
   long opt_force_grid = 0;
-  long opt_ew_min_bytes = 0;  // stage-1 launches of at least this many bytes run the emit-warp build of the kernel (0: never, the
-                              // default: on H100 that build was slower at every launch size from 256 MiB to 1 GiB)
   long opt_host_skip_scan = 0;  // tuning: the host-pointer pipeline copies only (no scan launches; results are meaningless)
   long opt_copy_threads = 4;        // 0: no staging (cudaMemcpyAsync straight from the caller's memory)
   long opt_ring_slots = 8;
@@ -206,24 +201,25 @@ uint32_t *launch_ticket(sjb200_ctx *c, int parity) { return c->d_ticket + 4 * pa
 uint32_t *launch_flags(sjb200_ctx *c, int parity) { return parity ? c->d_flags + 1 + kCarrySlots : c->d_flags; }
 unsigned long long *launch_desc(sjb200_ctx *c, int parity) { return c->d_count_desc + size_t(parity) * c->desc_tiles; }
 
-bool make_tensor_map(sjb200_ctx *c, CUtensorMap *map, const uint8_t *d_buf, size_t len, bool *usable, int box_rows = kScan4BoxRows) {
+// the tensor map every scan kernel reads through: 4 KiB boxes of 32 rows of 128 bytes
+bool make_tensor_map(sjb200_ctx *c, CUtensorMap *map, const uint8_t *d_buf, size_t len, bool *usable) {
   memset(map, 0, sizeof(*map));
   *usable = false;
   const uint64_t rows = len / 128;
   if (!c->opt_use_tma || c->encode == nullptr || rows == 0) return true;
   if ((reinterpret_cast<uintptr_t>(d_buf) & 15u) != 0) return true;  // TMA needs a 16-byte aligned base
-  // A map is a function of (base, rows, box) alone; re-encoding it costs ~1 us of host time per document, which a batch
+  // A map is a function of (base, rows) alone; re-encoding it costs ~1 us of host time per document, which a batch
   // call of many documents pays before its first launch.  Recently encoded maps are kept in a small direct-mapped cache.
   const uintptr_t key = reinterpret_cast<uintptr_t>(d_buf);
-  TmapCacheEntry &ce = c->tmap_cache[((key >> 4) ^ (key >> 12) ^ rows ^ uint64_t(box_rows)) % kTmapCacheEntries];
-  if (ce.base == d_buf && ce.rows == rows && ce.box_rows == box_rows) {
+  TmapCacheEntry &ce = c->tmap_cache[((key >> 4) ^ (key >> 12) ^ rows) % kTmapCacheEntries];
+  if (ce.base == d_buf && ce.rows == rows) {
     *map = ce.map;
     *usable = true;
     return true;
   }
   cuuint64_t dims[2] = {128, rows};
   cuuint64_t strides[1] = {128};
-  cuuint32_t box[2] = {128, (cuuint32_t)box_rows};
+  cuuint32_t box[2] = {128, (cuuint32_t)kScan4BoxRows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = c->encode(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<uint8_t *>(d_buf), dims, strides, box, estr,
                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -234,27 +230,18 @@ bool make_tensor_map(sjb200_ctx *c, CUtensorMap *map, const uint8_t *d_buf, size
   }
   ce.base = d_buf;
   ce.rows = rows;
-  ce.box_rows = box_rows;
   ce.map = *map;
   *usable = true;
   return true;
 }
 
-// stage 1 and minify run on the scan4 structure (sjb200_scan4.cuh), validate_utf8 on utf8v2 (sjb200_utf8.cuh)
-bool use_scan4(const sjb200_ctx *, int kind) { return kind == kIndex || kind == kMinify; }
-// the one tensor map the kernel selected for `kind` reads through (scan4: 4 KiB boxes; the tile-synchronous kernels: 32 KiB)
-bool map_for(sjb200_ctx *c, int kind, CUtensorMap *map, const uint8_t *d_buf, size_t len, bool *usable) {
-  (void)kind;  // every kernel reads 4 KiB boxes of 32 rows
-  return make_tensor_map(c, map, d_buf, len, usable, kScan4BoxRows);
-}
-int grid_cap(sjb200_ctx *c, int kind) {
-  (void)kind;
+int grid_cap(sjb200_ctx *c) {
   if (c->grid4 == 0) c->grid4 = scan4_max_ctas_per_sm() * c->sm_count;
   return c->opt_grid > 0 ? int(c->opt_grid) : c->grid4;
 }
-int grid_for(sjb200_ctx *c, int kind, uint32_t nelements) {
+int grid_for(sjb200_ctx *c, uint32_t nelements) {
   if (c->opt_force_grid > 0) return int(c->opt_force_grid);  // tuning: a full grid even for a tiny document (measures the fixed cost of a launch)
-  return int(std::max<uint32_t>(1, std::min<uint32_t>(uint32_t(grid_cap(c, kind)), nelements)));
+  return int(std::max<uint32_t>(1, std::min<uint32_t>(uint32_t(grid_cap(c)), nelements)));
 }
 
 // where a sharded launch publishes its record (sjb200_comm), and the kind the record carries
@@ -309,7 +296,7 @@ bool enqueue_scan(sjb200_ctx *c, int kind, const CUtensorMap *map, bool tma, con
   p.carry_in = (carry_in_slot < 0) ? nullptr : c->d_carry + carry_in_slot;
   p.write_sentinels = write_sentinels ? 1u : 0u;
   p.carry_out = external_out ? external_out : c->d_carry + carry_out_slot;
-  p.carry_out_host = use_scan4(c, kind) ? host_out : nullptr;
+  p.carry_out_host = host_out;
   p.flags = c->d_flags;
   p.count_desc = c->d_count_desc;
   p.ticket = c->d_ticket;
@@ -328,30 +315,16 @@ bool enqueue_scan(sjb200_ctx *c, int kind, const CUtensorMap *map, bool tma, con
   }
   cudaEvent_t e1 = timed ? time_begin(c, stream) : nullptr;
   bool launched;
-  if (use_scan4(c, kind)) {
-    const uint32_t tpe = uint32_t(scan4_tiles_per_element());
-    const uint32_t nelem = (ntiles + tpe - 1) / tpe;
-    const int grid = grid_for(c, kind, nelem);
-    const bool ew = kind == kIndex && c->opt_ew_min_bytes > 0 && uint64_t(ntiles) * kTileBytes >= uint64_t(c->opt_ew_min_bytes);
-    if (ew || scan4_parks_in_global()) {  // emit warps: the parked masks wait in an L2-resident ring of the context
-      const size_t need = std::max(ew ? scan4_ew_park_words(grid_cap(c, kind)) : 0, scan4_parks_in_global() ? scan4_park_words(grid_cap(c, kind)) : 0);
-      if (c->d_park_words < need) {
-        cudaStreamSynchronize(c->stream);
-        cudaFree(c->d_park); c->d_park = nullptr; c->d_park_words = 0;
-        if (!dev_alloc(c, &c->d_park, need, "cudaMalloc(park)")) return false;
-        c->d_park_words = need;
-      }
-      p.park = c->d_park;
-    }
-    launched = ew ? ok(c, launch_scan4_ew(map, p, grid, stream), "launch scan4 (emit warps)") : ok(c, launch_scan4(map, p, grid, kind == kMinify ? 2 : 0, stream), "launch scan4");
-    c->ew_launches += (launched && ew) ? 1 : 0;
-  } else {
+  if (kind == kUtf8) {  // validate_utf8: utf8v2 (sjb200_utf8.cuh); stage 1 and minify: scan4 (sjb200_scan4.cuh)
     if (c->grid_u == 0) c->grid_u = utf8v2_max_ctas_per_sm() * c->sm_count;
     const uint64_t nblocks = (uint64_t(ntiles) * kTileBytes + 4095) / 4096;
     const uint64_t want = (nblocks + uint64_t(utf8v2_warps_per_cta()) - 1) / uint64_t(utf8v2_warps_per_cta());
     const int grid = c->opt_force_grid > 0 ? int(c->opt_force_grid) : int(std::max<uint64_t>(1, std::min<uint64_t>(uint64_t(c->opt_grid > 0 ? c->opt_grid : c->grid_u), want)));
-    p.carry_out_host = host_out;
     launched = ok(c, launch_utf8v2(map, p, grid, stream), "launch utf8v2");
+  } else {
+    const uint32_t tpe = uint32_t(scan4_tiles_per_element());
+    const uint32_t nelem = (ntiles + tpe - 1) / tpe;
+    launched = ok(c, launch_scan4(map, p, grid_for(c, nelem), kind == kMinify ? 2 : 0, stream), "launch scan4");
   }
   time_end(c, stream, e1, launched, 1);
   c->launches += launched ? 1 : 0;
@@ -450,7 +423,7 @@ extern "C" void sjb200_destroy(sjb200_ctx *c) {
   DeviceGuard g(c->device);
   if (c->stream) cudaStreamSynchronize(c->stream);
   free_sized(c);
-  cudaFree(c->d_carry); cudaFree(c->d_flags); cudaFree(c->d_ticket); cudaFree(c->d_sfin); cudaFree(c->d_doc_scratch); cudaFree(c->d_ndocs); cudaFree(c->d_tok_scratch); cudaFree(c->d_tok_tot); cudaFree(c->d_tails); cudaFree(c->d_tail_ptrs); cudaFree(c->d_debug); cudaFree(c->d_park); cudaFree(c->d_doctab); cudaFree(c->d_stamps);
+  cudaFree(c->d_carry); cudaFree(c->d_flags); cudaFree(c->d_ticket); cudaFree(c->d_sfin); cudaFree(c->d_doc_scratch); cudaFree(c->d_ndocs); cudaFree(c->d_tok_scratch); cudaFree(c->d_tok_tot); cudaFree(c->d_tails); cudaFree(c->d_tail_ptrs); cudaFree(c->d_debug); cudaFree(c->d_doctab); cudaFree(c->d_stamps);
   if (c->h_doctab) cudaFreeHost(c->h_doctab);
   if (c->h_carry) cudaFreeHost(c->h_carry);
   if (c->h_flags) cudaFreeHost(c->h_flags);
@@ -536,8 +509,7 @@ extern "C" double sjb200_get_stat(sjb200_ctx *c, const char *key) {
     return n ? sum / double(n) : -1.0;
   }
   if (!strcmp(key, "launches")) return double(c->launches);
-  if (!strcmp(key, "ew_launches")) return double(c->ew_launches);
-  if (!strcmp(key, "grid_index")) return double(grid_for(c, kIndex, 0xFFFFFFFFu));
+  if (!strcmp(key, "grid_index")) return double(grid_for(c, 0xFFFFFFFFu));
   if (!strcmp(key, "sm_count")) return double(c->sm_count);
   if (!strcmp(key, "host_wait_ms")) return c->t_wait_ms;
   if (!strcmp(key, "xchg_polls")) return double(c->xchg_polls);
@@ -563,7 +535,6 @@ extern "C" int sjb200_set_option(sjb200_ctx *c, const char *key, long value) {
   else if (!strcmp(key, "launch_stamps")) c->opt_launch_stamps = value ? 1 : 0;
   else if (!strcmp(key, "chunk_bytes")) c->opt_chunk_bytes = std::max<long>(2 * kTileBytes, (value / (2 * kTileBytes)) * (2 * kTileBytes));
   else if (!strcmp(key, "force_grid")) c->opt_force_grid = value;
-  else if (!strcmp(key, "ew_min_bytes")) c->opt_ew_min_bytes = value;
   else if (!strcmp(key, "host_skip_scan")) c->opt_host_skip_scan = value;
   else if (!strcmp(key, "copy_threads")) c->opt_copy_threads = std::max<long>(0, std::min<long>(value, 64));
   else if (!strcmp(key, "ring_slots")) c->opt_ring_slots = std::max<long>(2, std::min<long>(value, 64));
@@ -620,12 +591,10 @@ void stage1_enqueue_into(sjb200_ctx *c, PendingCall &pc, const uint8_t *d_buf, s
   if (!ensure_desc(c, len)) { pc.early_error = SJB200_MEMALLOC; return; }
   CUtensorMap map;
   bool tma = false;
-  map_for(c, kIndex, &map, d_buf, len, &tma);
-  // scan4 stores its result in the pinned host mirror itself; the older kernel needs the copy engine for it
+  make_tensor_map(c, &map, d_buf, len, &tma);
+  // the kernel stores its result in the pinned host mirror itself
   if (!enqueue_scan(c, kIndex, &map, tma, d_buf, len, 0, tiles_of(len), true, 0x20202020u, d_idx, nullptr, -1, s, slot, true, nullptr,
-                    c->h_carry + slot) ||
-      (!use_scan4(c, kIndex) &&
-       !ok(c, cudaMemcpyAsync(c->h_carry + slot, c->d_carry + slot, sizeof(Carry), cudaMemcpyDeviceToHost, s), "D2H result")))
+                    c->h_carry + slot))
     { pc.early_error = SJB200_UNEXPECTED_ERROR; return; }
   stage1_stream_epilogue(c, pc);
 }
@@ -769,7 +738,7 @@ int enqueue_doc_groups(sjb200_ctx *c, std::vector<PendingCall> &calls, cudaStrea
     for (size_t k = 0; k < n; k++) {
       const PendingCall &pc = calls[size_t(G[k])];
       bool tma = false;
-      map_for(c, kIndex, &hm[k], pc.d_buf, pc.len, &tma);
+      make_tensor_map(c, &hm[k], pc.d_buf, pc.len, &tma);
       DocEntry &e = he[k];
       e.buf = pc.d_buf;
       e.idx_out = pc.d_idx;
@@ -817,7 +786,7 @@ int enqueue_doc_groups(sjb200_ctx *c, std::vector<PendingCall> &calls, cudaStrea
       PendingCall &pc = calls[size_t(G[0])];
       CUtensorMap map;
       bool tma = false;
-      map_for(c, kIndex, &map, pc.d_buf, pc.len, &tma);
+      make_tensor_map(c, &map, pc.d_buf, pc.len, &tma);
       if (!enqueue_scan(c, kIndex, &map, tma, pc.d_buf, pc.len, 0, tiles_of(pc.len), true, 0x20202020u, pc.d_idx, nullptr, -1, s, pc.carry_slot, true,
                         nullptr, c->h_carry + pc.carry_slot, nullptr, false)) {
         pc.early_error = SJB200_UNEXPECTED_ERROR;
@@ -849,7 +818,7 @@ int enqueue_doc_groups(sjb200_ctx *c, std::vector<PendingCall> &calls, cudaStrea
     if (good) {
       CUtensorMap unused;
       memset(&unused, 0, sizeof(unused));
-      good = ok(c, launch_scan4(&unused, p, grid_for(c, kIndex, g_elems_of[g]), 0, s, pdl), "launch scan4 (documents)");
+      good = ok(c, launch_scan4(&unused, p, grid_for(c, g_elems_of[g]), 0, s, pdl), "launch scan4 (documents)");
       c->launches += good ? 1 : 0;
       timed_docs += good ? uint32_t(n) : 0u;
     }
@@ -1006,7 +975,7 @@ extern "C" int sjb200_minify_dev_enqueue(sjb200_ctx *c, const uint8_t *d_buf, si
   if (!ensure_desc(c, len)) { pc.early_error = SJB200_MEMALLOC; return SJB200_SUCCESS; }
   CUtensorMap map;
   bool tma = false;
-  map_for(c, kMinify, &map, d_buf, len, &tma);
+  make_tensor_map(c, &map, d_buf, len, &tma);
   if (!enqueue_scan(c, kMinify, &map, tma, d_buf, len, 0, tiles_of(len), true, 0x20202020u, nullptr, d_dst, -1, s, 1) ||
       !fetch_result(c, s))
     pc.early_error = SJB200_UNEXPECTED_ERROR;
@@ -1045,7 +1014,7 @@ extern "C" int sjb200_validate_utf8_dev_enqueue(sjb200_ctx *c, const uint8_t *d_
   if (len > kMaxBytes) { pc.early_error = SJB200_CAPACITY; return SJB200_SUCCESS; }
   CUtensorMap map;
   bool tma = false;
-  map_for(c, kUtf8, &map, d_buf, len, &tma);
+  make_tensor_map(c, &map, d_buf, len, &tma);
   if (!enqueue_scan(c, kUtf8, &map, tma, d_buf, len, 0, tiles_of(len), true, 0x20202020u, nullptr, nullptr, -1, s, 1) ||
       !fetch_result(c, s))
     pc.early_error = SJB200_UNEXPECTED_ERROR;
@@ -1165,7 +1134,7 @@ bool scan_host_document(sjb200_ctx *c, int kind, const uint8_t *buf, size_t len,
   c->last_output_path = direct_out ? 1 : 0;
   CUtensorMap map;
   bool tma = false;
-  map_for(c, kind, &map, c->d_in, len, &tma);
+  make_tensor_map(c, &map, c->d_in, len, &tma);
   // calls are synchronous, so no earlier kernel still reads d_in when the first copy lands
   auto launch_chunk = [&](size_t k, const uint8_t *src) -> bool {
     const size_t off = bounds[k];
@@ -1178,9 +1147,6 @@ bool scan_host_document(sjb200_ctx *c, int kind, const uint8_t *buf, size_t len,
     if (c->opt_host_skip_scan) return true;
     if (!enqueue_scan(c, kind, &map, tma, c->d_in, len, uint32_t(off / kTileBytes), tiles_of(bytes), last, 0x20202020u, d_idx, d_dst,
                       k == 0 ? -1 : int(k), c->stream, int(k + 1), false, nullptr, c->h_carry + k + 1))
-      return false;
-    if (!use_scan4(c, kind) &&  // scan4 mirrors its result to the pinned host slot itself
-        !ok(c, cudaMemcpyAsync(c->h_carry + k + 1, c->d_carry + k + 1, sizeof(Carry), cudaMemcpyDeviceToHost, c->stream), "D2H carry"))
       return false;
     return !drain || ok(c, cudaEventRecord(scanned, c->stream), "event record");
   };
@@ -1269,7 +1235,7 @@ extern "C" int sjb200_stage1(sjb200_ctx *c, const uint8_t *buf, size_t len, int 
     if (len == 0) return SJB200_UTF8_ERROR;
   }
   DeviceGuard g(c->device);
-  uint32_t *alias = use_scan4(c, kIndex) ? mapped_alias(c, idx_out) : nullptr;
+  uint32_t *alias = mapped_alias(c, idx_out);
   if (!ensure_input(c, len) || (!alias && !ensure_index(c, len)) || !ensure_desc(c, len)) return SJB200_MEMALLOC;
   int slot = 0;
   if (!scan_host_document(c, kIndex, buf, len, alias ? alias : c->d_idx, nullptr, idx_out, sizeof(uint32_t), alias != nullptr, &slot))
@@ -1337,7 +1303,7 @@ extern "C" int sjb200_stage1_shard_dev(sjb200_ctx *c, const uint8_t *d_buf, size
   if (!ensure_desc(c, len)) return SJB200_MEMALLOC;
   CUtensorMap map;
   bool tma = false;
-  map_for(c, kIndex, &map, d_buf, len, &tma);
+  make_tensor_map(c, &map, d_buf, len, &tma);
   c->h_carry[0].count = 0; c->h_carry[0].state = state_in & 7u; c->h_carry[0].ttable = 0;
   (void)last_shard;  // every shard checks its own end: cuts are at character boundaries (sjb200_shard_cut)
   c->h_carry[0].flags = 0; c->h_carry[0].reserved = 0;
@@ -1363,7 +1329,7 @@ extern "C" int sjb200_stage1_shard_dev_enqueue(sjb200_ctx *c, const uint8_t *d_b
   if (!ensure_desc(c, len)) return SJB200_MEMALLOC;
   CUtensorMap map;
   bool tma = false;
-  map_for(c, kIndex, &map, d_buf, len, &tma);
+  make_tensor_map(c, &map, d_buf, len, &tma);
   if (!enqueue_scan(c, kIndex, &map, tma, d_buf, len, 0, tiles_of(len), true, 0x20202020u, d_idx, nullptr, -1, s, 1, false,
                     static_cast<Carry *>(d_result)))
     return SJB200_UNEXPECTED_ERROR;
@@ -1547,7 +1513,7 @@ int sharded_enqueue(sjb200_comm *m, int kind, const uint8_t *d_shard, size_t len
     len = trim_partial_utf8_tail(c->h_small, k, len);
   }
   const int scan_kind = idx_kind ? kIndex : kind;  // stream and delimited passes scan like stage 1; only their records' kind differs
-  if (use_scan4(c, scan_kind) && len && !ensure_desc(c, len)) return SJB200_MEMALLOC;
+  if (scan_kind != kUtf8 && len && !ensure_desc(c, len)) return SJB200_MEMALLOC;  // (scan4's look-back descriptors)
   const uint32_t seq = m->head + 1;  // tags start at 1: a zeroed window never matches
   XchgTarget x;
   for (int r = 0; r < kMaxRanks; r++) x.peer[r] = m->peer[r];
@@ -1566,7 +1532,7 @@ int sharded_enqueue(sjb200_comm *m, int kind, const uint8_t *d_shard, size_t len
   } else {
     CUtensorMap map;
     bool tma = false;
-    map_for(c, scan_kind, &map, d_shard, len, &tma);
+    make_tensor_map(c, &map, d_shard, len, &tma);
     good = enqueue_scan(c, scan_kind, &map, tma, d_shard, len, 0, tiles_of(len), true, 0x20202020u, d_idx, d_dst, -1, s, 1, false, m->d_result + i, nullptr, &x);
   }
   if (!good || !ok(c, cudaEventRecord(m->done[i], s), "event record"))
@@ -1582,7 +1548,7 @@ int minify_shard_from(sjb200_ctx *c, const uint8_t *d_buf, size_t len, uint32_t 
   if (!ensure_desc(c, len)) return SJB200_MEMALLOC;
   CUtensorMap map;
   bool tma = false;
-  map_for(c, kMinify, &map, d_buf, len, &tma);
+  make_tensor_map(c, &map, d_buf, len, &tma);
   c->h_carry[0].count = 0; c->h_carry[0].state = state_in & 7u; c->h_carry[0].ttable = 0;
   c->h_carry[0].flags = 0; c->h_carry[0].reserved = 0;
   if (!ok(c, cudaMemcpyAsync(c->d_carry, c->h_carry, sizeof(Carry), cudaMemcpyHostToDevice, s), "H2D carry") ||

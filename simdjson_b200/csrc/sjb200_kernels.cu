@@ -24,10 +24,8 @@
 
 namespace sjb200 {
 
-// ------------------------------------------------------------------ scan4 (stage 1; see sjb200_scan4.cuh)
-// two variants of one source: pipelined (masks wait in shared memory, an element is emitted two scans after it was scanned)
-// and deferred (masks wait in an L2-resident scratch ring, everything is emitted after the CTA's last scan: launches
-// small enough that every CTA holds all its elements at once never stall on the chain)
+// ------------------------------------------------------------------ scan4 (see sjb200_scan4.cuh)
+// one body, two modes: stage 1 (structural indexes + UTF-8 validation) and minify
 __global__ void __launch_bounds__(scan4::kThreads4, (SJB200_SCAN4_WARPS > 8) ? 1 : SJB200_SCAN4_MIN_CTAS)
     scan4_kernel(const __grid_constant__ CUtensorMap tmap, const ScanParams p) {
   extern __shared__ uint8_t smem_raw4[];
@@ -121,8 +119,6 @@ int utf8v2_max_ctas_per_sm() {
 }
 int utf8v2_warps_per_cta() { return utf8v2::kWarpsU; }
 
-size_t scan4_park_words(int grid) { return size_t(grid) * scan4::kParkRing * scan4::kParkSlotWords + 8; }
-int scan4_parks_in_global() { return scan4::kGPark > 0 ? 1 : 0; }
 int scan4_tiles_per_element() { return scan4::kElemBytes / kTileBytes; }
 
 int scan4_max_ctas_per_sm() {

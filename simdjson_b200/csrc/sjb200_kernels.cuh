@@ -15,13 +15,8 @@ namespace sjb200 {
 // launch, is still running (ScanParams::early_input)
 cudaError_t launch_scan4(const CUtensorMap *tmap, const ScanParams &p, int grid, int mode /*0 stage 1, 2 minify*/,
                          cudaStream_t stream, bool pdl = false);
-size_t scan4_park_words(int grid);   // uint32 words of ScanParams::park for a launch of `grid` CTAs (emit-warp builds)
 int scan4_tiles_per_element();      // 32 KiB tiles of the launch parameter block per scan4 element
-int scan4_parks_in_global();         // 1: every scan4 launch needs ScanParams::park (emit warps read the parked masks from an L2-resident ring)
 int scan4_max_ctas_per_sm();
-// the emit-warp build of the same kernel for large stage-1 launches (sjb200_kernels_ew.cu); always parks in ScanParams::park
-cudaError_t launch_scan4_ew(const CUtensorMap *tmap, const ScanParams &p, int grid, cudaStream_t stream);
-size_t scan4_ew_park_words(int grid);
 constexpr int kScan4BoxRows = 32;
 // utf8v2: validate_utf8 with independent warps (sjb200_utf8.cuh); same 32-row boxes
 cudaError_t launch_utf8v2(const CUtensorMap *tmap, const ScanParams &p, int grid, cudaStream_t stream);

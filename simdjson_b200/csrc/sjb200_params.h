@@ -68,11 +68,10 @@ struct ScanParams {
   uint32_t write_sentinels; // kIndex: the launch that scans the last tile also stores idx[n]=idx[n+1]=len, idx[n+2]=0
   const Carry *carry_in;    // null: zero state, zero count
   Carry *carry_out;
-  Carry *carry_out_host;    // scan4: optional second copy of the result in pinned host memory (saves the copy engine a trip between launches)
+  Carry *carry_out_host;    // optional second copy of the result in pinned host memory (saves the copy engine a trip between launches)
   uint32_t *flags;          // accumulated with atomicOr; zero between launches (the last CTA moves it to carry_out->flags)
   unsigned long long *count_desc;  // the look-back chain: one descriptor per scan4 element of the launch
   uint32_t *ticket;         // [0] next ticket, [1] CTAs finished, [2] scan4: aggregates published so far (4 words, zero between launches)
-  uint32_t *park;           // scan4 with emit warps: scratch ring for parked masks, scan4_park_words(grid) words (stays in L2)
   unsigned long long *debug;  // optional [ntiles][8] timeline (globaltimer ns) for tuning; null in production
   // multi-GPU exchange fused into the scan (scan4 and utf8v2): the launch's last CTA stores the shard record {count,
   // state out, transducer, flags, kind} into EVERY rank's exchange window over NVLink (peer-mapped device memory), tagged

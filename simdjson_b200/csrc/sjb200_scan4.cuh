@@ -24,8 +24,7 @@
 //     prefix and posts every block's polarity and output offset to the scan warps through an mbarrier.
 //   * Software pipeline: a scan warp emits element j-2 after scanning element j (per-lane bit loops into a
 //     shared-memory staging area -- the block buffer it has just consumed -- and coalesced 16-byte stores).  The TMA
-//     load of its next block is always in flight.  A second schedule ("deferred": masks parked in an L2-resident
-//     scratch ring, all emits after the CTA's last scan) is kept as an option.
+//     load of its next block is always in flight.
 //   * All arithmetic is the bit-plane algebra of sjb200_bits.cuh: 32 bytes per LOP3, no per-byte code.
 //   * Stage 1 may scan several whole documents in one launch (ScanParams::docs): tickets and descriptors run over the
 //     concatenation of their elements, every slot carries its element's document (Smem::tdoc), and each document is
@@ -49,37 +48,18 @@ constexpr int kScanWarps = SJB200_SCAN4_WARPS;  // scan warps per CTA = blocks p
 constexpr int kBlockBytes = 4096;
 constexpr int kBlockRows = kBlockBytes / 128;
 constexpr int kChainWarps = 1;  // the warp that resolves this CTA's elements
-#ifndef SJB200_SCAN4_EMITW
-#define SJB200_SCAN4_EMITW 0
-#endif
-// Emit warps (stage 1 only): the scan is bound by the ALU pipe, the emit by FLO / shared-memory latency.  When the warp
-// that scanned a block also emits it, all warps of the CTA sit in the emit loop together, with the ALU pipe
-// nearly idle.  Dedicated warps take resolved blocks from a CTA-wide queue
-// and emit them while the scan warps go on scanning.  0: every scan warp emits its own blocks (minify always does).
-constexpr int kEmitWarps = SJB200_SCAN4_EMITW;
-constexpr int kThreads4 = 32 * (kScanWarps + kChainWarps + kEmitWarps);
+constexpr int kThreads4 = 32 * (kScanWarps + kChainWarps);
 #ifndef SJB200_SCAN4_PARK
 #define SJB200_SCAN4_PARK 3
 #endif
 constexpr int kPark = SJB200_SCAN4_PARK;  // elements whose masks wait in shared memory: a scan warp emits element j-kLag after scanning j
 constexpr int kLag = kPark - 1;
 constexpr int kNS = 32;          // ring of element slots (tickets, summaries, resolutions)
-constexpr int kParkSlotWords = 2 * kScanWarps * 32 * 4 + kScanWarps * 32;  // one element's parked words (both polarities + prefixes)
-#ifndef SJB200_SCAN4_GPARK
-#define SJB200_SCAN4_GPARK 8
-#endif
-// With emit warps the parked masks may wait in an L2-resident scratch ring in global memory (ScanParams::park) instead of
-// shared memory: the emit warps do not care about the extra latency, and the ring can be deep -- the scan warps then
-// never wait for the chain as long as an element is resolved and emitted within kGPark - 1 scans (with three elements
-// parked in shared memory, every hiccup of the look-back chain stalled the scan).  0: park in shared memory.
-constexpr int kGPark = (SJB200_SCAN4_EMITW > 0) ? SJB200_SCAN4_GPARK : 0;
-constexpr int kParkRing = (kGPark > 0) ? kGPark : 1;  // slots per CTA of the global scratch ring
-constexpr int kParkFree = (kGPark > 0) ? kGPark : kPark;   // elements whose masks may be parked at once (emit-warp mode)
 #ifndef SJB200_SCAN4_LOOKK
 #define SJB200_SCAN4_LOOKK 10
 #endif
 constexpr int kLookK = SJB200_SCAN4_LOOKK;       // descriptors per lane and look-back round trip (window of 320 elements >= one wave of CTAs)
-static_assert(kLag >= 1 && 2 * kLag + 3 <= kNS && 2 * kGPark + 4 <= kNS && (kNS & (kNS - 1)) == 0, "slot ring");
+static_assert(kLag >= 1 && 2 * kLag + 3 <= kNS && (kNS & (kNS - 1)) == 0, "slot ring");
 #ifndef SJB200_SCAN4_TRACE
 #define SJB200_SCAN4_TRACE 0  // 1: tuning build that records where a scan warp's time goes (shared memory, dumped to ScanParams::debug at exit)
 #endif
@@ -102,9 +82,8 @@ enum : uint32_t { kDescNone = 0, kDescAgg = 1, kDescInc = 2 };
 
 struct Smem {
   uint8_t ring[kScanWarps][2][kBlockBytes];   // per scan warp: two block buffers (TMA destination / emit staging)
-  uint8_t estage[kEmitWarps > 0 ? kEmitWarps : 1][kBlockBytes];  // emit warps: staging areas (1 KiB aligned like the ring: minify fetches blocks into them by TMA)
-  sj_u4 park[kGPark > 0 ? 1 : kPark][2][kGPark > 0 ? 1 : kScanWarps * 32];  // [pipeline buffer][polarity][thread]: candidate structural masks (shared-memory parking)
-  uint32_t parkpre[kGPark > 0 ? 1 : kPark][kGPark > 0 ? 1 : kScanWarps * 32];  // exclusive prefix of the lane's counts inside its block, both polarities packed
+  sj_u4 park[kPark][2][kScanWarps * 32];      // [pipeline buffer][polarity][thread]: candidate structural masks
+  uint32_t parkpre[kPark][kScanWarps * 32];   // exclusive prefix of the lane's counts inside its block, both polarities packed
   uint32_t compact_lut[16];                   // minify: see compact_entry
   alignas(16) DocEntry doc[kMaxLaunchDocs];   // the launch's documents (a single-document launch: entry 0 from ScanParams)
   uint32_t ndocs;
@@ -120,12 +99,6 @@ struct Smem {
   sj_mbar_t ticket_ready[kNS];
   sj_mbar_t scanned[kNS];
   sj_mbar_t resolved[kNS];
-  // emit warps
-  sj_mbar_t efull[kEmitWarps > 0 ? kEmitWarps : 1];  // minify: completion of an emit warp's block fetch
-  sj_mbar_t park_free[kParkFree];  // phase k: every block of element (slot + k * kParkFree) has been emitted, the parked masks may be overwritten
-  uint32_t emitted_cnt[kNS];     // blocks of the element emitted so far
-  uint32_t emit_next;            // next (element, block) item: element = item / kScanWarps
-  uint32_t scan_done;            // 0xFFFFFFFF while the scan warps are running, then the number of elements this CTA scanned
 #if SJB200_SCAN4_TRACE
   uint32_t trace[2][kTraceIters][kTracePoints];  // tuning build: SM cycle counter at the phase boundaries of scan warps 0 and 9
   unsigned long long trace_cta[4];               // globaltimer: kernel entry, roles start, scan role done, before exit
@@ -580,15 +553,12 @@ SJ_DEV void emit_block(Smem *S, const ScanParams &p, uint64_t out_base, uint32_t
   if (!SJB200_SCAN4_TRACE && p.debug != nullptr && warp == 0 && lane == 0) p.debug[uint64_t(elem) * 8 + 5] = sj_globaltimer();
 }
 
-// pipelined mode: the masks wait in shared memory
+// emit_block with the lane's masks parked in shared memory
 SJ_DEV void emit_from_smem(Smem *S, const ScanParams &p, uint64_t out_base, uint32_t e, unsigned warp, unsigned lane, uint32_t *stg) {
   const uint32_t pol = S->res_pol[e % kNS][warp] & 1u;
   const unsigned tid = warp * 32 + lane;
-  emit_block(S, p, out_base, e, warp, lane, S->park[kGPark > 0 ? 0 : e % kPark][pol][kGPark > 0 ? 0 : tid], S->parkpre[kGPark > 0 ? 0 : e % kPark][kGPark > 0 ? 0 : tid], stg);
+  emit_block(S, p, out_base, e, warp, lane, S->park[e % kPark][pol][tid], S->parkpre[e % kPark][tid], stg);
 }
-
-// emit-warp mode: the masks wait in the scratch ring of ScanParams::park (it stays in L2)
-SJ_DEV uint32_t *park_slot(const ScanParams &p, uint32_t e) { return p.park + (size_t(sj_cta()) * kParkRing + (e % uint32_t(kParkRing))) * size_t(kParkSlotWords); }
 
 // ------------------------------------------------------------------------------------------------ minify: emit one block
 // kept bytes of a 4-byte word packed to its low end: the PRMT selector (unused positions select a zero byte)
@@ -794,10 +764,6 @@ SJ_DEV bool issue_load(Smem *S, uint32_t d, const ScanParams &p, uint32_t le, un
   return full;
 }
 
-template <int kMode>
-SJ_DEV void emit_role(Smem *S, const sj_tensor_map *tmap, const ScanParams &p, const Carry &cin, unsigned lane, uint8_t *stage, sj_mbar_t *fetch_bar,
-                      uint32_t fetch_phase);
-
 // kMode: 0 stage 1; 2 minify
 template <int kMode>
 SJ_DEV void scan_role(Smem *S, const sj_tensor_map *tmap, const ScanParams &p, const Carry &cin, unsigned warp, unsigned lane, uint32_t first_ticket) {
@@ -827,7 +793,6 @@ SJ_DEV void scan_role(Smem *S, const sj_tensor_map *tmap, const ScanParams &p, c
   }
   uint32_t ne = 0;  // this CTA's next element to emit (elements are emitted in order)
   uint32_t j = 0;
-  constexpr bool kEmitW = (kEmitWarps > 0);  // the emit warps take the blocks from here: this warp only scans
   for (;; j++) {
     if (t >= nelem) break;
     const int r = int(j & 1u);
@@ -869,25 +834,15 @@ SJ_DEV void scan_role(Smem *S, const sj_tensor_map *tmap, const ScanParams &p, c
       const uint32_t pw0 = sj_shfl(pw_cur, 0);
       const uint32_t st = boundary_state(D.buf, bstart, launch_start, cin.state, pw0, lane);
       SJ_TRACE4(4);
-      {
-        // the parked masks of element j - kParkFree must have been emitted before this element's take their place
-        if (kEmitW && j >= uint32_t(kParkFree)) wait_bar(&S->park_free[j % kParkFree], ((j / kParkFree) - 1u) & 1u, p, 64);
-        const uint64_t left = D.len - bstart;  // > 0: bytes of the block that exist
-        const uint32_t valid = left < uint64_t(kBlockBytes) ? uint32_t(left) : uint32_t(kBlockBytes);
-        if (kEmitW && kGPark > 0) {
-          uint32_t *slot = park_slot(p, j);
-          summary = scan_block<kMin>(T, pw0, st & 1u, (st >> 2) & 1u, lane, D.flags, reinterpret_cast<sj_u4 *>(slot), reinterpret_cast<sj_u4 *>(slot) + kScanWarps * 32,
-                                     slot + 2 * kScanWarps * 32 * 4, valid);
-        } else {
-          summary = scan_block<kMin>(T, pw0, st & 1u, (st >> 2) & 1u, lane, D.flags, S->park[j % kPark][0], S->park[j % kPark][1], S->parkpre[j % kPark], valid);
-        }
-      }
+      const uint64_t left = D.len - bstart;  // > 0: bytes of the block that exist
+      const uint32_t valid = left < uint64_t(kBlockBytes) ? uint32_t(left) : uint32_t(kBlockBytes);
+      summary = scan_block<kMin>(T, pw0, st & 1u, (st >> 2) & 1u, lane, D.flags, S->park[j % kPark][0], S->park[j % kPark][1], S->parkpre[j % kPark], valid);
     }
     if (!SJB200_SCAN4_TRACE && p.debug != nullptr && warp == 0 && lane == 0) p.debug[uint64_t(t) * 8 + 1] = sj_globaltimer();
     // minify: the slot just scanned is free -- ask for the block that is emitted below now, the fetch (L2) runs while the
     // element is composed and resolved
     int fetched = -1;
-    if (kMin && !kEmitW && j >= uint32_t(kLag)) fetched = minify_fetch_issue(S, tmap, p, ne, warp, lane, T, &S->full[warp][r], launch_start) ? 1 : 0;
+    if (kMin && j >= uint32_t(kLag)) fetched = minify_fetch_issue(S, tmap, p, ne, warp, lane, T, &S->full[warp][r], launch_start) ? 1 : 0;
     SJ_TRACE4(5);
     {
       const int ns = int(j % kNS);
@@ -909,14 +864,14 @@ SJ_DEV void scan_role(Smem *S, const sj_tensor_map *tmap, const ScanParams &p, c
     }
     SJ_TRACE4(6);
     SJ_TRACE4(7);
-    if (!kEmitW && j >= uint32_t(kLag)) {  // pipelined: the chain warp has had kLag scans' time to resolve this one
+    if (j >= uint32_t(kLag)) {  // the chain warp has had kLag scans' time to resolve this one
       if (j == uint32_t(kLag)) wait_previous_launch();  // the first emit: the previous launch may write the same index array
       wait_bar(&S->resolved[ne % kNS], (ne / kNS) & 1u, p, 64);
       SJ_TRACE4(8);
       if (!SJB200_SCAN4_TRACE && p.debug != nullptr && warp == 0 && lane == 0) p.debug[uint64_t(S->ticket[ne % kNS]) * 8 + 2] = sj_globaltimer();
       if (kMin) {
         const uint32_t pol = S->res_pol[ne % kNS][warp] & 1u;
-        if (emit_minify_block(S, tmap, p, out_base, ne, warp, lane, S->park[kGPark > 0 ? 0 : ne % kPark][pol][kGPark > 0 ? 0 : warp * 32 + lane], S->parkpre[kGPark > 0 ? 0 : ne % kPark][kGPark > 0 ? 0 : warp * 32 + lane], T,
+        if (emit_minify_block(S, tmap, p, out_base, ne, warp, lane, S->park[ne % kPark][pol][warp * 32 + lane], S->parkpre[ne % kPark][warp * 32 + lane], T,
                               &S->full[warp][r], (full_phase >> r) & 1u, launch_start, fetched))
           full_phase ^= 1u << r;
       } else {
@@ -930,81 +885,18 @@ SJ_DEV void scan_role(Smem *S, const sj_tensor_map *tmap, const ScanParams &p, c
     pw_cur = pw_next;
   }
   // drain: what this CTA scanned and has not emitted yet (no load is in flight: both ring slots are free)
-  if (kEmitW) {
-    if (warp == 0 && lane == 0) sj_st_release_u32(&S->scan_done, j);  // the emit warps stop after element j - 1
-    sj_syncwarp();
-    // nothing left to scan: help with what is left to emit (both ring slots are free: slot 0 is the staging area)
-    emit_role<kMode>(S, tmap, p, cin, lane, S->ring[warp][0], &S->full[warp][0], full_phase & 1u);
-  } else {
-    if (ne < j) wait_previous_launch();  // (the CTA scanned kLag elements or fewer: nothing emitted yet)
-    while (ne < j) {
-      wait_bar(&S->resolved[ne % kNS], (ne / kNS) & 1u, p, 64);
-      if (kMin) {
-        const uint32_t pol = S->res_pol[ne % kNS][warp] & 1u;
-        if (emit_minify_block(S, tmap, p, out_base, ne, warp, lane, S->park[kGPark > 0 ? 0 : ne % kPark][pol][kGPark > 0 ? 0 : warp * 32 + lane], S->parkpre[kGPark > 0 ? 0 : ne % kPark][kGPark > 0 ? 0 : warp * 32 + lane],
-                              S->ring[warp][0], &S->full[warp][0], full_phase & 1u, launch_start))
-          full_phase ^= 1u;
-      } else {
-        emit_from_smem(S, p, out_base, ne, warp, lane, reinterpret_cast<uint32_t *>(S->ring[warp][0]));
-      }
-      ne++;
-    }
-  }
-}
-
-// ------------------------------------------------------------------------------------------------ emit warps
-// Items are (element, block) pairs in the order the CTA scanned them; a warp takes the next item, waits until the
-// element is resolved, emits the block exactly as the scanning warp would have (same parked words, same staging scheme,
-// its own staging area), and reports it.  The last block of an element frees the element's parked masks.
-template <int kMode>
-SJ_DEV void emit_role(Smem *S, const sj_tensor_map *tmap, const ScanParams &p, const Carry &cin, unsigned lane, uint8_t *stage, sj_mbar_t *fetch_bar,
-                      uint32_t fetch_phase) {  // stage: this warp's 4 KiB staging area; minify fetches blocks into it through fetch_bar (next parity: fetch_phase)
-  const uint64_t out_base = cin.count;
-  const uint64_t launch_start = uint64_t(p.tile_begin) * kTileBytes;
-  uint32_t *stg = reinterpret_cast<uint32_t *>(stage);
-  wait_previous_launch();  // before the first emit
-  for (;;) {
-    uint32_t q = 0;
-    if (lane == 0) q = sj_atomic_add(&S->emit_next, 1u);
-    q = sj_shfl(q, 0);
-    const uint32_t e = q / uint32_t(kScanWarps), b = q % uint32_t(kScanWarps);
-    // until element e is resolved -- or the scan warps report that this CTA never drew an element e
-    uint32_t spins = 0;
-    for (;;) {
-      if (sj_mbar_try_wait(&S->resolved[e % kNS], (e / kNS) & 1u)) break;
-      const uint32_t done = sj_ld_acquire_u32(&S->scan_done);
-      if (done != 0xFFFFFFFFu && e >= done) return;
-      if (spun_out(&spins)) {
-        sj_atomic_or(p.flags, kFlagInternal);
-        return;
-      }
-      sj_nanosleep(32);
-    }
-    const uint32_t pol = S->res_pol[e % kNS][b] & 1u;
-    const unsigned tid = b * 32u + lane;
-    sj_u4 ev;
-    uint32_t prew;
-    if (kGPark > 0) {
-      const uint32_t *slot = park_slot(p, e);
-      ev = sj_ld_u4(slot + (pol * kScanWarps * 32 + tid) * 4);
-      prew = sj_ld_u32(slot + 2 * kScanWarps * 32 * 4 + tid);
+  if (ne < j) wait_previous_launch();  // (the CTA scanned kLag elements or fewer: nothing emitted yet)
+  while (ne < j) {
+    wait_bar(&S->resolved[ne % kNS], (ne / kNS) & 1u, p, 64);
+    if (kMin) {
+      const uint32_t pol = S->res_pol[ne % kNS][warp] & 1u;
+      if (emit_minify_block(S, tmap, p, out_base, ne, warp, lane, S->park[ne % kPark][pol][warp * 32 + lane], S->parkpre[ne % kPark][warp * 32 + lane],
+                            S->ring[warp][0], &S->full[warp][0], full_phase & 1u, launch_start))
+        full_phase ^= 1u;
     } else {
-      ev = S->park[kGPark > 0 ? 0 : e % kPark][pol][kGPark > 0 ? 0 : tid];
-      prew = S->parkpre[kGPark > 0 ? 0 : e % kPark][kGPark > 0 ? 0 : tid];
+      emit_from_smem(S, p, out_base, ne, warp, lane, reinterpret_cast<uint32_t *>(S->ring[warp][0]));
     }
-    if (kMode == 2) {
-      if (emit_minify_block(S, tmap, p, out_base, e, b, lane, ev, prew, stage, fetch_bar, fetch_phase, launch_start)) fetch_phase ^= 1u;
-    } else {
-      emit_block(S, p, out_base, e, b, lane, ev, prew, stg);
-    }
-    sj_syncwarp();
-    if (lane == 0) {
-      sj_fence_block();
-      if (sj_atomic_add(&S->emitted_cnt[e % kNS], 1u) == uint32_t(kScanWarps - 1)) {
-        S->emitted_cnt[e % kNS] = 0;
-        sj_mbar_arrive(&S->park_free[e % kParkFree]);
-      }
-    }
+    ne++;
   }
 }
 
@@ -1215,26 +1107,17 @@ SJ_DEV void scan4_body(const sj_tensor_map *tmap, const ScanParams &p, uint8_t *
   cin.count = 0; cin.state = 0; cin.ttable = 0; cin.flags = 0; cin.reserved = 0;
   if (p.carry_in != nullptr) cin = *p.carry_in;
   if (tid == 0 && p.stamps != nullptr && first_ticket == 0) p.stamps[0] = t_entry;
-  // ~140 mbarriers: one thread each (a single thread initialising them all is slow)
+  // 128 mbarriers: one thread each (a single thread initialising them all is slow)
   if (tid < unsigned(kNS)) {
     sj_mbar_init(&S->ticket_ready[tid], 1);
     sj_mbar_init(&S->scanned[tid], 1);
     sj_mbar_init(&S->resolved[tid], 1);
     S->arrived[tid] = 0;
-    S->emitted_cnt[tid] = 0;
   } else if (tid < unsigned(kNS + 2 * kScanWarps)) {
     const unsigned k = tid - unsigned(kNS);
     sj_mbar_init(&S->full[k >> 1][k & 1u], 1);
-  } else if (tid < unsigned(kNS + 2 * kScanWarps + kParkFree)) {
-    sj_mbar_init(&S->park_free[tid - unsigned(kNS + 2 * kScanWarps)], 1);
-  } else if (tid < unsigned(kNS + 2 * kScanWarps + kParkFree + (kEmitWarps > 0 ? kEmitWarps : 1))) {
-    sj_mbar_init(&S->efull[tid - unsigned(kNS + 2 * kScanWarps + kParkFree)], 1);
   }
-  if (tid == 0) {
-    S->emit_next = 0;
-    S->scan_done = 0xFFFFFFFFu;
-  }
-  if (tid < unsigned(kNS + 2 * kScanWarps + kParkFree + (kEmitWarps > 0 ? kEmitWarps : 1))) sj_fence_mbar_init();
+  if (tid < unsigned(kNS + 2 * kScanWarps)) sj_fence_mbar_init();
   if (kMode == 2 && tid < 16) S->compact_lut[tid] = compact_entry(tid);
   if (p.ndocs > 0) {  // the document table, 16 bytes per thread
     const uint32_t nw = p.ndocs * uint32_t(sizeof(DocEntry) / 16);
@@ -1261,8 +1144,7 @@ SJ_DEV void scan4_body(const sj_tensor_map *tmap, const ScanParams &p, uint8_t *
   if (tid == 0) S->trace_cta[1] = sj_globaltimer();
 #endif
   if (warp < unsigned(kScanWarps)) scan_role<kMode>(S, tmap, p, cin, warp, lane, first_ticket);
-  else if (warp < unsigned(kScanWarps + kChainWarps)) chain_role(S, p, cin, lane, warp - unsigned(kScanWarps));
-  else emit_role<kMode>(S, tmap, p, cin, lane, S->estage[warp - unsigned(kScanWarps + kChainWarps)], &S->efull[warp - unsigned(kScanWarps + kChainWarps)], 0u);
+  else chain_role(S, p, cin, lane, warp - unsigned(kScanWarps));
 #if SJB200_SCAN4_TRACE
   if (tid == 0) S->trace_cta[2] = sj_globaltimer();
 #endif

@@ -69,8 +69,6 @@ SJ_DEV sj_u4 sj_make_u4(uint32_t x, uint32_t y, uint32_t z, uint32_t w) { sj_u4 
 SJ_DEV sj_u4 sj_ldg_u4(const void *p) { sj_u4 v; memcpy(&v, p, 16); return v; }
 SJ_DEV uint32_t sj_ldg_u32(const void *p) { uint32_t v; memcpy(&v, p, 4); return v; }
 SJ_DEV uint32_t sj_ldg_u8(const uint8_t *p) { return *p; }
-SJ_DEV sj_u4 sj_ld_u4(const void *p) { sj_u4 v; memcpy(&v, p, 16); return v; }
-SJ_DEV uint32_t sj_ld_u32(const void *p) { uint32_t v; memcpy(&v, p, 4); return v; }
 
 SJ_DEV unsigned sj_tid() { return simt::tctx.tid; }
 SJ_DEV unsigned sj_cta() { return simt::tctx.cta; }
@@ -145,8 +143,6 @@ SJ_DEV void sj_st_sys_u64(unsigned long long *p, unsigned long long v) { __atomi
 SJ_DEV void sj_fence_gpu_release() { __atomic_thread_fence(__ATOMIC_SEQ_CST); }
 SJ_DEV uint32_t sj_ld_relaxed_u32(const uint32_t *p) { return __atomic_load_n(p, __ATOMIC_ACQUIRE); }
 SJ_DEV void sj_fence_block() { __atomic_thread_fence(__ATOMIC_SEQ_CST); }
-SJ_DEV void sj_st_release_u32(uint32_t *p, uint32_t v) { __atomic_store_n(p, v, __ATOMIC_RELEASE); }
-SJ_DEV uint32_t sj_ld_acquire_u32(const uint32_t *p) { return __atomic_load_n(p, __ATOMIC_ACQUIRE); }
 SJ_DEV void sj_nanosleep(unsigned) {
   struct timespec ts = {0, 20000};
   nanosleep(&ts, nullptr);
@@ -263,9 +259,6 @@ SJ_DEV sj_u4 sj_make_u4(uint32_t x, uint32_t y, uint32_t z, uint32_t w) { return
 SJ_DEV sj_u4 sj_ldg_u4(const void *p) { return __ldg(reinterpret_cast<const uint4 *>(p)); }
 SJ_DEV uint32_t sj_ldg_u32(const void *p) { return __ldg(reinterpret_cast<const uint32_t *>(p)); }
 SJ_DEV uint32_t sj_ldg_u8(const uint8_t *p) { return __ldg(p); }
-// data written earlier by this same kernel (the parked masks): plain loads, not the read-only path
-SJ_DEV sj_u4 sj_ld_u4(const void *p) { return *reinterpret_cast<const uint4 *>(p); }
-SJ_DEV uint32_t sj_ld_u32(const void *p) { return *reinterpret_cast<const uint32_t *>(p); }
 
 SJ_DEV unsigned sj_tid() { return threadIdx.x; }
 SJ_DEV unsigned sj_cta() { return blockIdx.x; }
@@ -314,16 +307,6 @@ SJ_DEV uint32_t sj_ld_relaxed_u32(const uint32_t *p) {
   return v;
 }
 SJ_DEV void sj_fence_block() { __threadfence_block(); }
-// a flag in shared memory between warps of one CTA
-SJ_DEV void sj_st_release_u32(uint32_t *p, uint32_t v) {
-  __threadfence_block();
-  *reinterpret_cast<volatile uint32_t *>(p) = v;
-}
-SJ_DEV uint32_t sj_ld_acquire_u32(const uint32_t *p) {
-  const uint32_t v = *reinterpret_cast<const volatile uint32_t *>(p);
-  __threadfence_block();
-  return v;
-}
 SJ_DEV void sj_nanosleep(unsigned ns) { __nanosleep(ns); }
 SJ_DEV unsigned sj_smid() {
   unsigned r;

@@ -96,7 +96,6 @@ void emu_launch(unsigned grid, const sj_tensor_map &tmap, const ScanParams &p, i
 // what sjb200_capi.cu keeps per context
 struct EmuCtx {
   std::vector<unsigned long long> desc;
-  std::vector<uint32_t> park;
   uint32_t ticket[4] = {0, 0, 0, 0};
   uint32_t flags = 0;
   uint32_t epoch = 0;
@@ -142,8 +141,6 @@ Result run_scan4(EmuCtx &cx, const uint8_t *buf, size_t len, uint32_t state_in, 
     p.flags = &cx.flags; p.count_desc = cx.desc.data(); p.ticket = cx.ticket; p.debug = nullptr;
     cx.carry[slot + 1] = Carry();
     const unsigned g = std::min<unsigned>(grid, (nt * unsigned(kTileBytes) + scan4::kElemBytes - 1) / scan4::kElemBytes);
-    cx.park.assign(size_t(g) * scan4::kParkRing * scan4::kParkSlotWords + 8, 0xDEADBEEFu);
-    p.park = reinterpret_cast<uint32_t *>((reinterpret_cast<uintptr_t>(cx.park.data()) + 15) & ~uintptr_t(15));
     emu_launch(g, tmap, p, minify_dst ? 2 : 0);
     if (cx.ticket[0] != 0 || cx.ticket[1] != 0 || cx.ticket[2] != 0 || cx.flags != 0) { fprintf(stderr, "BUG: ticket/flags not re-armed\n"); exit(2); }
     flags |= cx.carry[slot + 1].flags;
@@ -265,8 +262,7 @@ int test_look_back(std::mt19937_64 &rng, int cases) {
     }
     ScanParams p;
     memset(&p, 0, sizeof(p));
-    uint32_t tick[4] = {0, 0, t, 0};  // (the published-aggregates counter of the SJB200_SCAN4_COUNTER build option)
-    p.epoch = epoch; p.count_desc = desc.data(); p.flags = &flags; p.ticket = tick;
+    p.epoch = epoch; p.count_desc = desc.data(); p.flags = &flags;
     simt::WarpShared w;
     simt::CtaShared cta;
     pthread_barrier_init(&w.bar, nullptr, 32);

@@ -96,7 +96,6 @@ void emu_launch(unsigned grid, const sj_tensor_map &tmap, const ScanParams &p, i
 constexpr size_t kWindowWords = size_t(kXchgSteps) * 2 * kMaxRanks * 2;
 struct EmuJob {
   std::vector<unsigned long long> desc;
-  std::vector<uint32_t> park;
   uint32_t ticket[4] = {0, 0, 0, 0};
   uint32_t flags = 0;
   uint32_t epoch = 0;
@@ -147,8 +146,6 @@ Carry launch_shard(EmuJob &J, int kind, const uint8_t *buf, size_t len, uint32_t
   p.write_sentinels = kind == kIndex ? 1u : 0u;
   p.count_desc = J.desc.data();
   g = std::min<unsigned>(grid, unsigned((uint64_t(ntiles) * kTileBytes + scan4::kElemBytes - 1) / scan4::kElemBytes));
-  J.park.assign(size_t(g) * scan4::kParkRing * scan4::kParkSlotWords + 8, 0xDEADBEEFu);
-  p.park = reinterpret_cast<uint32_t *>((reinterpret_cast<uintptr_t>(J.park.data()) + 15) & ~uintptr_t(15));
   emu_launch(g, tmap, p, kind == kMinify ? 2 : 0);
   EXPECT(J.ticket[0] == 0 && J.ticket[1] == 0 && J.ticket[2] == 0 && J.flags == 0, "scan4 ticket/flags not re-armed");
   return J.carry[1];
