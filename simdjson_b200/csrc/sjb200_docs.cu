@@ -164,12 +164,12 @@ __global__ void __launch_bounds__(kFinishThreads) stream_finish_kernel(const uin
 // into every rank's window at word `at` (this rank's block).  kept = the shard's structurals, less the stream's last one
 // when the stream ends inside a string and this shard holds it; walk = 0 (regular mode) skips the walk.
 __global__ void __launch_bounds__(kFinishThreads) stream_summary_kernel(const uint8_t *buf, const uint32_t *idx, uint32_t count, uint32_t kept, uint32_t len,
-                                                                       int walk, ScanParams x, size_t at) {
+                                                                       int walk, const __grid_constant__ Xchg x, size_t at) {
   __shared__ int sh[kFinishThreads / 32];
   int start = -1, nobj = 0, narr = 0;
   if (walk && kept > 0) last_document_start(buf, idx, kept, sh, &start, &nobj, &narr);
   const uint32_t r = threadIdx.x;
-  if (r < x.xchg_nranks) {
+  if (r < x.nranks) {
     uint32_t w[kSumWords];
     w[0] = len;
     w[1] = count ? idx[0] : 0u;
@@ -179,9 +179,9 @@ __global__ void __launch_bounds__(kFinishThreads) stream_summary_kernel(const ui
     w[5] = uint32_t(nobj);
     w[6] = uint32_t(narr);
     w[7] = (kept ? role_of(buf[idx[0]]) | (role_of(buf[idx[kept - 1]]) << 3) : 0u) | (start >= 0 ? 1u << 6 : 0u);
-    unsigned long long *rec = x.xchg_peer[r] + at;
+    unsigned long long *rec = x.peer[r] + at;
     for (int k = 0; k < kSumWords; k++) {
-      const unsigned long long v = (static_cast<unsigned long long>(x.xchg_seq) << 32) | w[k];
+      const unsigned long long v = (static_cast<unsigned long long>(x.seq) << 32) | w[k];
       asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(rec + k), "l"(v) : "memory");
     }
   }
@@ -515,12 +515,12 @@ __global__ void __launch_bounds__(kFinishThreads) filter_finish_kernel(const uin
 }
 
 // ---------------------------------------------------------------------------------------------- sharded RS / comma passes
-// the extra rounds of a delimited pass (sjb200_capi.cu): every kernel stores its words, tagged with x.xchg_seq, into
+// the extra rounds of a delimited pass (sjb200_comm.cu): every kernel stores its words, tagged with x.seq, into
 // every rank's window at word `at` (this rank's block, sjb200_params.h)
-__device__ __forceinline__ void store_tagged(const ScanParams &x, uint32_t r, size_t at, const uint32_t *w, int nwords) {
-  unsigned long long *rec = x.xchg_peer[r] + at;
+__device__ __forceinline__ void store_tagged(const Xchg &x, uint32_t r, size_t at, const uint32_t *w, int nwords) {
+  unsigned long long *rec = x.peer[r] + at;
   for (int k = 0; k < nwords; k++) {
-    const unsigned long long v = (static_cast<unsigned long long>(x.xchg_seq) << 32) | w[k];
+    const unsigned long long v = (static_cast<unsigned long long>(x.seq) << 32) | w[k];
     asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(rec + k), "l"(v) : "memory");
   }
 }
@@ -542,9 +542,9 @@ __global__ void __launch_bounds__(kWsThreads) trailing_ws_kernel(const uint8_t *
 // structurals (*depth_total); RS: whether it ends inside a separator run (its last structural is an RS entry followed
 // only by whitespace / RS, *other == 0) and whether it is whitespace / RS only
 __global__ void delim_carry_kernel(const uint8_t *buf, const uint32_t *idx, uint32_t n, uint32_t len, int comma, const int *depth_total, const int *other,
-                                   ScanParams x, size_t at) {
+                                   const __grid_constant__ Xchg x, size_t at) {
   const bool ok = comma || *other == 0;
-  if (threadIdx.x < x.xchg_nranks) {
+  if (threadIdx.x < x.nranks) {
     uint32_t w[kDelimCarryWords];
     w[0] = len;
     w[1] = comma ? uint32_t(*depth_total) : uint32_t(n > 0 && buf[idx[n - 1]] == 0x1E && ok);
@@ -562,17 +562,17 @@ __global__ void delim_totals_kernel(const uint32_t *dst, const int *kept_total, 
   out4[0] = n; out4[1] = seps; out4[2] = last_sep; out4[3] = lo;
 }
 
-__global__ void publish_kernel(const uint32_t *src, uint32_t nwords, ScanParams x, size_t at) {
-  if (threadIdx.x < x.xchg_nranks) store_tagged(x, threadIdx.x, at, src, int(nwords));
+__global__ void publish_kernel(const uint32_t *src, uint32_t nwords, const __grid_constant__ Xchg x, size_t at) {
+  if (threadIdx.x < x.nranks) store_tagged(x, threadIdx.x, at, src, int(nwords));
 }
 
 // tail round: the (at most three) words n, n+1, n+2 of the whole call this rank holds, read before the filtered entries
 // go back into idx -- a word past the filtered array is what the scan left there (a raw structural, as after the
 // reference's in-place filter)
-__global__ void delim_tail_kernel(const uint32_t *dst, const uint32_t *idx, DelimTail t, ScanParams x, size_t at) {
+__global__ void delim_tail_kernel(const uint32_t *dst, const uint32_t *idx, DelimTail t, const __grid_constant__ Xchg x, size_t at) {
   uint32_t w[3];
   for (int k = 0; k < 3; k++) w[k] = t.src[k] == 1 ? dst[t.pos[k]] + t.add : (t.src[k] == 2 ? idx[t.pos[k]] + t.add : 0u);
-  if (threadIdx.x < x.xchg_nranks) store_tagged(x, threadIdx.x, at, w, 3);
+  if (threadIdx.x < x.nranks) store_tagged(x, threadIdx.x, at, w, 3);
 }
 
 struct FilterScratch {
@@ -651,7 +651,7 @@ cudaError_t launch_doc_table(const uint8_t *buf, const uint32_t *idx, uint32_t n
   return cudaGetLastError();
 }
 
-cudaError_t launch_stream_summary(const uint8_t *buf, const uint32_t *idx, uint32_t count, uint32_t kept, uint32_t len, int walk, const ScanParams &x,
+cudaError_t launch_stream_summary(const uint8_t *buf, const uint32_t *idx, uint32_t count, uint32_t kept, uint32_t len, int walk, const Xchg &x,
                                   size_t at, cudaStream_t stream) {
   stream_summary_kernel<<<1, kFinishThreads, 0, stream>>>(buf, idx, count, kept, len, walk, x, at);
   return cudaGetLastError();
@@ -659,7 +659,7 @@ cudaError_t launch_stream_summary(const uint8_t *buf, const uint32_t *idx, uint3
 
 size_t delim_scratch_words(uint32_t n) { return filter_scratch_words(n) + 8; }
 
-cudaError_t launch_delim_carry(const uint8_t *buf, const uint32_t *idx, uint32_t n, uint32_t len, bool comma, uint32_t *scratch, const ScanParams &x,
+cudaError_t launch_delim_carry(const uint8_t *buf, const uint32_t *idx, uint32_t n, uint32_t len, bool comma, uint32_t *scratch, const Xchg &x,
                                size_t at, cudaStream_t stream) {
   const FilterScratch f = filter_layout(scratch, n);
   const uint32_t ntiles = (n + kFltTile - 1) / kFltTile;
@@ -703,12 +703,12 @@ cudaError_t launch_delim_filter(const uint8_t *buf, uint32_t len, const uint32_t
 
 const uint32_t *delim_filtered(const uint32_t *scratch) { return scratch; }
 
-cudaError_t launch_delim_publish_totals(uint32_t *scratch, uint32_t n, const ScanParams &x, size_t at, cudaStream_t stream) {
+cudaError_t launch_delim_publish_totals(uint32_t *scratch, uint32_t n, const Xchg &x, size_t at, cudaStream_t stream) {
   publish_kernel<<<1, 32, 0, stream>>>(filter_layout(scratch, n).out4, 4, x, at);
   return cudaGetLastError();
 }
 
-cudaError_t launch_delim_tail(uint32_t *scratch, uint32_t n, uint32_t *idx, const DelimTail &t, bool publish, const ScanParams &x, size_t at,
+cudaError_t launch_delim_tail(uint32_t *scratch, uint32_t n, uint32_t *idx, const DelimTail &t, bool publish, const Xchg &x, size_t at,
                               cudaStream_t stream) {
   const FilterScratch f = filter_layout(scratch, n);
   if (publish) delim_tail_kernel<<<1, 32, 0, stream>>>(f.dst, idx, t, x, at);

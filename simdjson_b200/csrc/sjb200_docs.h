@@ -34,9 +34,9 @@ cudaError_t launch_stream_filter(const uint8_t *buf, uint32_t len, uint32_t *idx
 size_t doc_table_scratch_words(uint32_t n);
 cudaError_t launch_doc_table(const uint8_t *buf, const uint32_t *idx, uint32_t n, bool first_starts, uint32_t *scratch, sjb200_doc_boundary_t *table,
                              uint32_t capacity, uint32_t *ndocs_dev, cudaStream_t stream);
-// sharded streaming passes: the shard's summary into every rank's window (fields xchg_* of x; layout in sjb200_params.h)
+// sharded streaming passes: the shard's summary into every rank's window (x; layout in sjb200_params.h)
 // (at: the word of this rank's block in every window)
-cudaError_t launch_stream_summary(const uint8_t *buf, const uint32_t *idx, uint32_t count, uint32_t kept, uint32_t len, int walk, const ScanParams &x,
+cudaError_t launch_stream_summary(const uint8_t *buf, const uint32_t *idx, uint32_t count, uint32_t kept, uint32_t len, int walk, const Xchg &x,
                                   size_t at, cudaStream_t stream);
 // ... and the rewrite of the (at most two) words of the final fix-up this rank holds
 cudaError_t launch_store_words(uint32_t *idx, uint32_t nw, uint32_t p0, uint32_t v0, uint32_t p1, uint32_t v1, cudaStream_t stream);
@@ -46,14 +46,14 @@ cudaError_t launch_store_words(uint32_t *idx, uint32_t nw, uint32_t p0, uint32_t
 // scratch: delim_scratch_words(n) words, kept from the carry round to the tail round
 size_t delim_scratch_words(uint32_t n);
 // carry round
-cudaError_t launch_delim_carry(const uint8_t *buf, const uint32_t *idx, uint32_t n, uint32_t len, bool comma, uint32_t *scratch, const ScanParams &x,
+cudaError_t launch_delim_carry(const uint8_t *buf, const uint32_t *idx, uint32_t n, uint32_t len, bool comma, uint32_t *scratch, const Xchg &x,
                                size_t at, cudaStream_t stream);
 // filter round: the filter with the carried-in depth / run into the scratch (idx untouched); {filtered, separators, last
 // separator, filtered before it} -> totals_host (pinned, valid once the stream is synchronised)
 cudaError_t launch_delim_filter(const uint8_t *buf, uint32_t len, const uint32_t *idx, uint32_t n, bool comma, int depth_in, bool run_in, uint32_t *scratch,
                                 uint32_t *totals_host, cudaStream_t stream);
 const uint32_t *delim_filtered(const uint32_t *scratch);  // the filtered entries, shard-relative
-cudaError_t launch_delim_publish_totals(uint32_t *scratch, uint32_t n, const ScanParams &x, size_t at, cudaStream_t stream);
+cudaError_t launch_delim_publish_totals(uint32_t *scratch, uint32_t n, const Xchg &x, size_t at, cudaStream_t stream);
 // tail round: the words this rank holds (src 1: filtered entry pos, 2: raw scanned word pos, 0: none; + add), published when
 // `publish`; then the filtered entries go back to idx[0, filtered)
 struct DelimTail {
@@ -61,7 +61,7 @@ struct DelimTail {
   uint32_t pos[3];
   uint32_t add;
 };
-cudaError_t launch_delim_tail(uint32_t *scratch, uint32_t n, uint32_t *idx, const DelimTail &t, bool publish, const ScanParams &x, size_t at,
+cudaError_t launch_delim_tail(uint32_t *scratch, uint32_t n, uint32_t *idx, const DelimTail &t, bool publish, const Xchg &x, size_t at,
                               cudaStream_t stream);
 
 }  // namespace sjb200

@@ -1,0 +1,265 @@
+// sjb200_fold.cpp -- the pure host folds of the sharded passes (sjb200_stream_fold, sjb200_delimited_fold) and the shard
+// helpers of include/sjb200.h that need no device.  No CUDA: the CPU tests drive these through ctypes.
+#include <stdint.h>
+#include <string.h>
+
+#include <algorithm>
+
+#include "../../include/sjb200.h"
+#include "sjb200_bits.cuh"
+#include "sjb200_common.h"
+#include "sjb200_params.h"
+
+using namespace sjb200;
+
+namespace {
+enum : uint32_t { kRoleValue = 0, kRoleSep, kRoleOpenObj, kRoleCloseObj, kRoleOpenArr, kRoleCloseArr };  // as in sjb200_docs.cu
+bool starts_document(uint32_t cur, uint32_t before) {  // find_next_document_index.h L60-88
+  if (cur == kRoleSep || cur == kRoleCloseObj || cur == kRoleCloseArr) return false;
+  return !(before == kRoleOpenObj || before == kRoleOpenArr || before == kRoleSep);
+}
+}  // namespace
+
+// The fold of the summaries into the whole stream's finish() (json_structural_indexer.h L249-343, L395-396).  T = all
+// structurals, n0 = T less the stream's last one when it ends inside a string (streaming modes).  The last document start
+// g of [0, n0) is the last internal start of the last shard that has one, unless the first structural of a later shard
+// starts a document across its cut; the brackets from g on are that shard's nets after its start plus the later shards'
+// nets.  Then m = n0 when they balance, else g (0 without any start), as find_next_document_index.
+extern "C" int sjb200_stream_fold(int mode, int nranks, uint32_t final_state, uint32_t flags_all, const sjb200_stream_summary *sums,
+                                  sjb200_stream_fold_result *res, sjb200_stream_rank *ranks) {
+  if (!res || !ranks || !sums || nranks < 1 || nranks > kMaxRanks || mode < SJB200_REGULAR || mode > SJB200_STREAMING_FINAL) return SJB200_UNEXPECTED_ERROR;
+  memset(res, 0, sizeof(*res));
+  memset(ranks, 0, sizeof(*ranks) * size_t(nranks));
+  uint64_t base[kMaxRanks], off = 0, T = 0;
+  int holder = -1;
+  for (int r = 0; r < nranks; r++) {
+    ranks[r].bytes_before = off;
+    off += sums[r].len;
+    base[r] = T;
+    T += sums[r].count;
+    if (sums[r].count) holder = r;
+  }
+  const uint64_t L = off;
+  res->total_bytes = L;
+  const bool streaming = mode != SJB200_REGULAR, unclosed = (final_state >> 1) & 1u;
+  auto done = [&](int err) {
+    res->error = err;
+    for (int r = 0; r < nranks && res->n_written; r++) {
+      const uint64_t k = res->n > base[r] ? res->n - base[r] : 0;
+      ranks[r].kept = std::min<uint64_t>(k, sums[r].count);
+    }
+    for (int r = 0, prev = -1; r < nranks; r++) {  // prev: the last earlier shard with kept structurals
+      if (ranks[r].kept == 0) continue;
+      ranks[r].first_starts_document = (prev < 0) ? 1u : uint32_t(starts_document(sums[r].role_first, sums[prev].role_last));
+      prev = r;
+    }
+    return err;
+  };
+  if (flags_all & kFlagInternal) return done(SJB200_UNEXPECTED_ERROR);
+  if (streaming && L == 0) return done(SJB200_UTF8_ERROR);           // L198-204: nothing left after the trim
+  if (!streaming && unclosed) return done(SJB200_UNCLOSED_STRING);   // L255-259
+  if (flags_all & kFlagCtl) return done(SJB200_UNESCAPED_CHARS);    // L261-263
+  res->n_written = 1;
+  res->n = T;
+  if (T == 0) return done(SJB200_EMPTY);                             // L289-291
+  const bool utf8 = (flags_all & kFlagUtf8) != 0;
+  if (!streaming) return done(utf8 ? SJB200_UTF8_ERROR : SJB200_SUCCESS);
+  const uint64_t n0 = T - (unclosed ? 1 : 0);
+  if (mode == SJB200_STREAMING_PARTIAL && unclosed && n0 == 0) { res->n = 0; return done(SJB200_CAPACITY); }  // L298-302
+  // the last document start g < n0 and the bracket balance of [g, n0); gv = global byte of structural g
+  uint64_t g = 0, gv = 0;
+  bool found = false;
+  int64_t nobj = 0, narr = 0;
+  for (int r = nranks - 1; r >= 0 && !found; r--) {
+    const uint64_t kp = sums[r].count - ((unclosed && r == holder) ? 1 : 0);
+    if (kp == 0) continue;
+    nobj += sums[r].net_obj;
+    narr += sums[r].net_arr;
+    if (sums[r].has_start) {
+      found = true; g = base[r] + sums[r].start_index; gv = ranks[r].bytes_before + sums[r].start_byte;
+    } else if (base[r] > 0) {
+      int q = r - 1;
+      while (q >= 0 && sums[q].count == 0) q--;
+      if (q >= 0 && starts_document(sums[r].role_first, sums[q].role_last)) { found = true; g = base[r]; gv = ranks[r].bytes_before + sums[r].first_byte; }
+    }
+  }
+  if (!found && n0 > 0) {  // the start is structural 0
+    int r0 = 0;
+    while (sums[r0].count == 0) r0++;
+    gv = ranks[r0].bytes_before + sums[r0].first_byte;
+  }
+  const uint64_t m = (n0 == 0) ? 0 : ((nobj == 0 && narr == 0) ? n0 : g);
+  if (mode == SJB200_STREAMING_PARTIAL) {  // L303-317
+    if (m == 0) {
+      const bool idx0_zero = sums[0].count > 0 && sums[0].first_byte == 0;
+      if (idx0_zero) { res->n = n0; return done(SJB200_CAPACITY); }
+      res->n = 0;
+      return done(SJB200_EMPTY);
+    }
+    res->n = m;
+    return done(utf8 ? SJB200_UTF8_ERROR : SJB200_SUCCESS);
+  }
+  // streaming final, L329-343: word m + 1 = old word m, word m = L; the ranks that hold them store them shard-relative
+  uint64_t old_m;
+  if (m >= T) old_m = L;                                                            // a sentinel
+  else if (m == T - 1 && unclosed) old_m = ranks[holder].bytes_before + sums[holder].last_byte;  // the dropped quote
+  else old_m = gv;                                                                  // a document start
+  const uint64_t pos[2] = {m, m + 1}, val[2] = {L, old_m};
+  for (int k = 0; k < 2; k++) {
+    int r = nranks - 1;
+    uint64_t local = sums[r].count + (pos[k] - T);
+    if (pos[k] < T) {
+      r = 0;
+      while (!(pos[k] >= base[r] && pos[k] < base[r] + sums[r].count)) r++;
+      local = pos[k] - base[r];
+    }
+    sjb200_stream_rank &w = ranks[r];
+    w.rewrite_pos[w.nrewrites] = uint32_t(local);
+    w.rewrite_val[w.nrewrites] = uint32_t(val[k] - w.bytes_before);
+    w.nrewrites++;
+  }
+  res->n = m;
+  if (m == 0) return done(SJB200_EMPTY);
+  return done(utf8 ? SJB200_UTF8_ERROR : SJB200_SUCCESS);
+}
+
+// The fold of a delimited pass's filter round into the whole stream's finish() for modes 3..6 (json_structural_indexer.h
+// L344-396 with find_next_document_index_json_sequence / filter_comma_delimited, as filter_finish_kernel runs it on one
+// GPU).  The filtered entries are sorted across the ranks, so the global last separator is the last one of the last
+// rank that counted any, and the entries before it are the filtered entries of the ranks before plus its `below`.
+// find_next_document_index over the first k filtered entries is sjb200_stream_fold's walk over the ranks' walk
+// summaries (every rank's full walk, the last rank's walk_below when k ends at its `below`).  The words after n are those
+// of the array the reference's in-place filter leaves: the filtered entries, then the scan's structurals, then the
+// sentinels len, len, 0.
+extern "C" int sjb200_delimited_fold(int mode, int nranks, uint32_t final_state, uint32_t flags_all, const sjb200_delimited_summary *sums,
+                                     sjb200_delimited_fold_result *res, sjb200_delimited_rank *ranks) {
+  if (!res || !ranks || !sums || nranks < 1 || nranks > kMaxRanks || mode < SJB200_JSON_SEQUENCE_PARTIAL || mode > SJB200_COMMA_DELIMITED_FINAL)
+    return SJB200_UNEXPECTED_ERROR;
+  memset(res, 0, sizeof(*res));
+  memset(ranks, 0, sizeof(*ranks) * size_t(nranks));
+  uint64_t base[kMaxRanks], off = 0, T = 0, W = 0, seps = 0;
+  int sep_rank = -1;  // the last rank that counted a separator
+  for (int r = 0; r < nranks; r++) {
+    ranks[r].bytes_before = off;
+    ranks[r].filtered_before = W;
+    off += sums[r].len;
+    base[r] = T;
+    T += sums[r].count;
+    W += sums[r].filtered;
+    seps += sums[r].seps;
+    if (sums[r].seps) sep_rank = r;
+  }
+  const uint64_t L = off;
+  res->total_bytes = L;
+  for (int k = 0; k < 3; k++) res->tail_rank[k] = -1;
+  const bool rs = (mode == SJB200_JSON_SEQUENCE_PARTIAL || mode == SJB200_JSON_SEQUENCE_FINAL);
+  const bool is_final = (mode == SJB200_JSON_SEQUENCE_FINAL || mode == SJB200_COMMA_DELIMITED_FINAL);
+  const bool unclosed = (final_state >> 1) & 1u;
+  auto word = [&](int k, uint64_t p) {  // word p of the array after the in-place filter -> tail k
+    if (p < W || p < T) {
+      const bool f = p < W;
+      int r = 0;
+      while (!(f ? (p >= ranks[r].filtered_before && p < ranks[r].filtered_before + sums[r].filtered) : (p >= base[r] && p < base[r] + sums[r].count))) r++;
+      res->tail_rank[k] = r;
+      res->tail_pos[k] = uint32_t(p - (f ? ranks[r].filtered_before : base[r]));
+      res->tail_filtered[k] = f ? 1u : 0u;
+    } else {
+      res->tail_val[k] = p < T + 2 ? uint32_t(L) : 0u;
+    }
+  };
+  auto words_from = [&](uint64_t p) { for (int k = 0; k < 3; k++) word(k, p + uint64_t(k)); };
+  auto done = [&](int err) {
+    res->error = err;
+    for (int r = 0; r < nranks && res->n_written; r++) {
+      const uint64_t k = res->n > ranks[r].filtered_before ? res->n - ranks[r].filtered_before : 0;
+      ranks[r].kept = std::min<uint64_t>(k, sums[r].filtered);
+    }
+    for (int r = 0, prev = -1; r < nranks; r++) {  // prev: the last earlier shard with kept entries
+      if (ranks[r].kept == 0) continue;
+      ranks[r].first_starts_document = (prev < 0) ? 1u : uint32_t(starts_document(sums[r].walk.role_first, sums[prev].walk.role_last));
+      prev = r;
+    }
+    return err;
+  };
+  // find_next_document_index over the first k filtered entries
+  auto walk = [&](uint64_t k) -> uint64_t {
+    sjb200_stream_summary ws[kMaxRanks];
+    for (int r = 0; r < nranks; r++) {
+      const uint64_t fb = ranks[r].filtered_before;
+      const uint64_t cnt = std::min<uint64_t>(k > fb ? k - fb : 0, sums[r].filtered);
+      if (cnt == 0) memset(&ws[r], 0, sizeof(ws[r]));
+      else ws[r] = (cnt == sums[r].filtered) ? sums[r].walk : sums[r].walk_below;
+      ws[r].count = cnt;
+      ws[r].len = sums[r].len;
+    }
+    sjb200_stream_fold_result fr;
+    sjb200_stream_rank fk[kMaxRanks];
+    sjb200_stream_fold(SJB200_STREAMING_FINAL, nranks, 0, 0, ws, &fr, fk);
+    return fr.n;
+  };
+  if (flags_all & kFlagInternal) return done(SJB200_UNEXPECTED_ERROR);
+  if (L == 0) return done(SJB200_UTF8_ERROR);                        // L198-204: nothing left after the trim
+  if (flags_all & kFlagCtl) return done(SJB200_UNESCAPED_CHARS);    // L261-263
+  res->n_written = 1;
+  res->n = T;
+  if (T == 0) { words_from(0); return done(SJB200_EMPTY); }          // L289-291
+  if (!is_final && unclosed && T == 1) { res->n = 0; words_from(0); return done(SJB200_CAPACITY); }  // L298-302, before the filter
+  uint64_t m = 0, n_res = W, next_start = L;
+  bool too_large = false;
+  const uint64_t last_sep = sep_rank >= 0 ? ranks[sep_rank].bytes_before + sums[sep_rank].last_sep : 0;
+  const uint64_t before_sep = sep_rank >= 0 ? ranks[sep_rank].filtered_before + sums[sep_rank].below : 0;
+  if (W != 0) {
+    if (rs) {
+      if (seps == 0) m = is_final ? walk(W) : 0;
+      else if (is_final) m = W;
+      else {
+        next_start = last_sep;
+        if (seps < 2) too_large = true;
+        else m = before_sep;
+      }
+    } else {
+      if (is_final) m = walk(W);
+      else if (seps == 0) too_large = true;
+      else {
+        next_start = last_sep + 1;
+        if (before_sep != 0) { n_res = before_sep; m = walk(before_sep); }
+      }
+    }
+  }
+  if (!is_final) {  // L344-359, L367-384
+    if (too_large) { res->n = n_res; words_from(n_res); return done(SJB200_CAPACITY); }
+    if (m == 0) { res->n = 0; words_from(0); return done(SJB200_EMPTY); }
+    res->n = m;
+    res->tail_val[0] = uint32_t(next_start);
+    word(1, m + 1);
+    word(2, m + 2);
+  } else {  // L360-366, L385-393: word m + 1 = the old word m
+    res->n = m;
+    res->tail_val[0] = uint32_t(L);
+    word(1, m);
+    word(2, m + 2);
+    if (m == 0) return done(SJB200_EMPTY);
+  }
+  return done((flags_all & kFlagUtf8) ? SJB200_UTF8_ERROR : SJB200_SUCCESS);
+}
+
+extern "C" uint32_t sjb200_fold_state(const uint32_t *ttables, int nshards_before) {
+  uint32_t state = 0;
+  for (int i = 0; i < nshards_before; i++) state = tt_apply(ttables[i], state);
+  return state;
+}
+
+extern "C" size_t sjb200_shard_cut(const uint8_t *buf, size_t len, size_t nominal) {
+  if (nominal >= len) return len;
+  size_t cut = nominal;
+  for (int k = 0; k < 3 && cut > 0 && (buf[cut] & 0xC0) == 0x80; k++) cut--;
+  return cut;
+}
+
+extern "C" size_t sjb200_shard_cut_line(const uint8_t *buf, size_t len, size_t nominal, size_t window) {
+  if (nominal >= len) return len;
+  const size_t lo = nominal > window ? nominal - window : 0;
+  for (size_t cut = nominal; cut > lo; cut--)
+    if (buf[cut - 1] == 0x0A) return cut;
+  return sjb200_shard_cut(buf, len, nominal);
+}

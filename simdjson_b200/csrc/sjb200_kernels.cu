@@ -61,10 +61,12 @@ __global__ void write_sentinels_kernel(uint32_t *idx, uint32_t n, uint32_t a, ui
 }
 
 // second round of a sharded pass (after re-scans): republish this rank's record in every rank's exchange window
-__global__ void xchg_post_kernel(ScanParams p, unsigned long long w0, unsigned long long w1) {
+// (x is __grid_constant__ here and in the exchange kernels of sjb200_docs.cu: x.peer[r] is then read from the parameter
+// space, not from a copy of x on the stack)
+__global__ void xchg_post_kernel(const __grid_constant__ Xchg x, unsigned long long w0, unsigned long long w1) {
   const uint32_t r = threadIdx.x;
-  if (r < p.xchg_nranks) {
-    unsigned long long *rec = p.xchg_peer[r] + (size_t(p.xchg_slot) * kMaxRanks + p.xchg_rank) * 2;
+  if (r < x.nranks) {
+    unsigned long long *rec = x.peer[r] + (size_t(x.slot) * kMaxRanks + x.rank) * 2;
     sj_st_sys_u64(rec, w0);
     sj_st_sys_u64(rec + 1, w1);
   }
@@ -134,8 +136,8 @@ cudaError_t launch_gather_tails(const uint8_t *const *bufs, const uint64_t *lens
   return cudaGetLastError();
 }
 
-cudaError_t launch_xchg_post(const ScanParams &p, unsigned long long w0, unsigned long long w1, cudaStream_t stream) {
-  xchg_post_kernel<<<1, 32, 0, stream>>>(p, w0, w1);
+cudaError_t launch_xchg_post(const Xchg &x, unsigned long long w0, unsigned long long w1, cudaStream_t stream) {
+  xchg_post_kernel<<<1, 32, 0, stream>>>(x, w0, w1);
   return cudaGetLastError();
 }
 

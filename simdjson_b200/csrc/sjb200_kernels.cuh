@@ -23,8 +23,8 @@ cudaError_t launch_utf8v2(const CUtensorMap *tmap, const ScanParams &p, int grid
 int utf8v2_max_ctas_per_sm();
 int utf8v2_warps_per_cta();
 cudaError_t launch_gather_tails(const uint8_t *const *bufs, const uint64_t *lens, uint32_t ndocs, uint8_t *out, cudaStream_t stream);
-// republish a shard record {w0, w1} in every rank's exchange window (fields xchg_* of p)
-cudaError_t launch_xchg_post(const ScanParams &p, unsigned long long w0, unsigned long long w1, cudaStream_t stream);
+// republish a shard record {w0, w1} in every rank's exchange window (x)
+cudaError_t launch_xchg_post(const Xchg &x, unsigned long long w0, unsigned long long w1, cudaStream_t stream);
 cudaError_t launch_write_sentinels(uint32_t *idx, uint32_t n, uint32_t a, uint32_t b, uint32_t c, cudaStream_t stream);
 
 }  // namespace sjb200

@@ -53,6 +53,16 @@ struct DocEntry {
 };
 constexpr int kMaxLaunchDocs = 64;  // documents per multi-document launch (their table is copied into every CTA's shared memory)
 
+// Where a launch of a sharded pass (sjb200_comm) stores its words: into EVERY rank's exchange window over NVLink
+// (peer-mapped device memory), each tagged with seq.  nranks == 0: no exchange.
+struct Xchg {
+  unsigned long long *peer[kMaxRanks];  // [r] = base of rank r's window (layout below)
+  uint32_t nranks, rank;
+  uint32_t slot;                        // the record slot of (seq, round): [slots][kMaxRanks][2] words
+  uint32_t seq;
+  uint32_t kind;                        // scan4 stage 1: the kind its record carries (kIndex, kStream or kDelim)
+};
+
 struct ScanParams {
   const uint8_t *buf;       // device pointer to byte 0 of the document (or shard)
   uint64_t len;             // document length in bytes (<= 4 GiB - 1); bytes past it read as 0x20
@@ -74,11 +84,9 @@ struct ScanParams {
   uint32_t *ticket;         // [0] next ticket, [1] CTAs finished, [2] scan4: aggregates published so far (4 words, zero between launches)
   unsigned long long *debug;  // optional [ntiles][8] timeline (globaltimer ns) for tuning; null in production
   // multi-GPU exchange fused into the scan (scan4 and utf8v2): the launch's last CTA stores the shard record {count,
-  // state out, transducer, flags, kind} into EVERY rank's exchange window over NVLink (peer-mapped device memory), tagged
-  // with xchg_seq -- the path's one exchange step (SURVEY.md 8e) without a collective launch.  xchg_nranks == 0: no exchange.
-  unsigned long long *xchg_peer[kMaxRanks];  // [r] = base of rank r's window: [slots][kMaxRanks][2] words
-  uint32_t xchg_nranks, xchg_rank, xchg_slot, xchg_seq;
-  uint32_t xchg_kind;       // scan4 stage 1: the kind its record carries (kIndex, kStream or kDelim)
+  // state out, transducer, flags, kind} into every rank's exchange window -- the path's one exchange step (SURVEY.md 8e)
+  // without a collective launch
+  Xchg xchg;
   // scan4 stage 1, several whole documents in one launch: ndocs (1..kMaxLaunchDocs) entries in device memory.  buf, len,
   // use_tma, idx_out, carry_out and carry_out_host are then unused; tile_begin = 0, no carry-in, no exchange, pos_base = 0,
   // prev_word = 0x20202020, check_eof = write_sentinels = 1, and `flags` only collects what concerns the whole launch.

@@ -1178,16 +1178,16 @@ SJ_DEV void scan4_body(const sj_tensor_map *tmap, const ScanParams &p, uint8_t *
         D.carry_out->flags = fl;
         if (D.carry_out_host != nullptr) D.carry_out_host->flags = fl;
       }
-      if (p.xchg_nranks != 0) {
+      if (p.xchg.nranks != 0) {
         // the exchange step of a sharded scan, fused: this launch's record goes straight into every rank's window
         // (finalize_launch's stores are visible here: its CTA fenced before it counted itself out)
         const volatile Carry *co = p.carry_out;
         // (minify validates nothing: of its flags only an internal error means something -- a shard cut inside a UTF-8
         // character or a control character in a string is not an error of minify)
-        const unsigned long long w0 = xchg_word0(p.xchg_seq, co->count),
-                                 w1 = xchg_word1(p.xchg_seq, co->state, co->ttable, kMode == 2 ? (fl & uint32_t(kFlagInternal)) : fl, kMode == 2 ? kMinify : int(p.xchg_kind));
-        for (uint32_t r = 0; r < p.xchg_nranks; r++) {
-          unsigned long long *rec = p.xchg_peer[r] + (size_t(p.xchg_slot) * kMaxRanks + p.xchg_rank) * 2;
+        const unsigned long long w0 = xchg_word0(p.xchg.seq, co->count),
+                                 w1 = xchg_word1(p.xchg.seq, co->state, co->ttable, kMode == 2 ? (fl & uint32_t(kFlagInternal)) : fl, kMode == 2 ? kMinify : int(p.xchg.kind));
+        for (uint32_t r = 0; r < p.xchg.nranks; r++) {
+          unsigned long long *rec = p.xchg.peer[r] + (size_t(p.xchg.slot) * kMaxRanks + p.xchg.rank) * 2;
           sj_st_sys_u64(rec, w0);
           sj_st_sys_u64(rec + 1, w1);
         }

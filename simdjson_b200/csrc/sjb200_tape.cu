@@ -185,21 +185,21 @@ __global__ void __launch_bounds__(1024) tile_scan_kernel(unsigned long long *til
     for (int w = 0; w < 32; w++) s += shs[w];
     tot->n_strings = s;
     tot->string_bytes = carry;
-    if (x.nranks != 0) {
+    if (x.xchg.nranks != 0) {
       const unsigned long long fe = tot->first_error;
       const uint32_t w[kSumWords] = {uint32_t(x.len), x.n, s, fe == ~0ull ? 0xFFFFFFFFu : uint32_t(fe >> 8), fe == ~0ull ? 0u : uint32_t(fe & 0xFFull),
                                      uint32_t(carry), uint32_t(carry >> 32), 0u};
-      const unsigned long long w0 = xchg_word0(x.seq, carry),
-                               w1 = xchg_word1(x.seq, x.state_in, 0, carry > x.capacity ? kTokShortFlag : 0u, kTokens);
+      const unsigned long long w0 = xchg_word0(x.xchg.seq, carry),
+                               w1 = xchg_word1(x.xchg.seq, x.state_in, 0, carry > x.capacity ? kTokShortFlag : 0u, kTokens);
 #pragma unroll
-      for (uint32_t r = 0; r < uint32_t(kMaxRanks); r++) {  // (unrolled: x.peer stays in the parameter space, no stack copy)
-        if (r >= x.nranks) break;
-        unsigned long long *sum = x.peer[r] + xchg_summary_at(x.seq, x.rank);
+      for (uint32_t r = 0; r < uint32_t(kMaxRanks); r++) {  // (unrolled: x.xchg.peer stays in the parameter space, no stack copy)
+        if (r >= x.xchg.nranks) break;
+        unsigned long long *sum = x.xchg.peer[r] + xchg_summary_at(x.xchg.seq, x.xchg.rank);
         for (int k = 0; k < kSumWords; k++) {
-          const unsigned long long v = (static_cast<unsigned long long>(x.seq) << 32) | w[k];
+          const unsigned long long v = (static_cast<unsigned long long>(x.xchg.seq) << 32) | w[k];
           asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(sum + k), "l"(v) : "memory");
         }
-        unsigned long long *rec = x.peer[r] + (size_t(x.slot) * kMaxRanks + x.rank) * 2;
+        unsigned long long *rec = x.xchg.peer[r] + (size_t(x.xchg.slot) * kMaxRanks + x.xchg.rank) * 2;
         asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(rec), "l"(w0) : "memory");
         asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(rec + 1), "l"(w1) : "memory");
       }

@@ -15,12 +15,11 @@ struct TokenTotals {
   uint32_t reserved;
 };
 
-// A sharded tokens pass (sjb200_comm): where tile_scan_kernel stores the shard's record (window slot `slot`, kind
+// A sharded tokens pass (sjb200_comm): where tile_scan_kernel stores the shard's record (window slot xchg.slot, kind
 // kTokens) and its summary (xchg_summary_at(seq, rank)) in every rank's window, and what they carry besides the totals.
-// nranks == 0: no exchange.
+// xchg.nranks == 0: no exchange.
 struct TokXchg {
-  unsigned long long *peer[kMaxRanks];
-  uint32_t nranks, rank, slot, seq;
+  Xchg xchg;
   uint32_t state_in;   // the scanner state the caller says the shard starts in (0: a clean cut)
   uint32_t n;
   uint64_t len;

@@ -12,7 +12,7 @@
 // units are transposed into bit planes and checked with the boolean rules of sjb200_bits.cuh, without further votes.
 // The three bytes before a lane's row come from the row before it (shared memory), those before a block from global
 // memory (one word, loaded one block ahead).  Errors are OR-ed in a register and reach memory once per warp.  In a sharded
-// pass (ScanParams::xchg_nranks != 0) the last CTA out also stores the shard's record into every rank's exchange window,
+// pass (ScanParams::xchg.nranks != 0) the last CTA out also stores the shard's record into every rank's exchange window,
 // as scan4 does (sjb200_validate_utf8_sharded*).
 //
 // Compiles for the host SIMT emulation as well (tests/simt_emul.cpp).
@@ -165,13 +165,13 @@ SJ_DEV void utf8_body(const sj_tensor_map *tmap, const ScanParams &p, uint8_t *s
         p.carry_out_host->ttable = 0;
         p.carry_out_host->flags = fl;
       }
-      if (p.xchg_nranks != 0) {
+      if (p.xchg.nranks != 0) {
         // sharded validate_utf8: this shard's record goes straight into every rank's window, as scan4 does.  Cuts are at
         // character boundaries, so a shard's verdict needs nothing from its neighbours: count, state and transducer are 0
         // and every rank folds state 0 (no second round); the ranks AND the verdicts (OR the flags).
-        const unsigned long long w0 = xchg_word0(p.xchg_seq, 0), w1 = xchg_word1(p.xchg_seq, 0, 0, fl, kUtf8);
-        for (uint32_t r = 0; r < p.xchg_nranks; r++) {
-          unsigned long long *rec = p.xchg_peer[r] + (size_t(p.xchg_slot) * kMaxRanks + p.xchg_rank) * 2;
+        const unsigned long long w0 = xchg_word0(p.xchg.seq, 0), w1 = xchg_word1(p.xchg.seq, 0, 0, fl, kUtf8);
+        for (uint32_t r = 0; r < p.xchg.nranks; r++) {
+          unsigned long long *rec = p.xchg.peer[r] + (size_t(p.xchg.slot) * kMaxRanks + p.xchg.rank) * 2;
           sj_st_sys_u64(rec, w0);
           sj_st_sys_u64(rec + 1, w1);
         }

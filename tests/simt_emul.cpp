@@ -93,7 +93,7 @@ void emu_launch(unsigned grid, const sj_tensor_map &tmap, const ScanParams &p, i
 }
 
 
-// what sjb200_capi.cu keeps per context
+// what the context keeps (sjb200_ctx.h)
 struct EmuCtx {
   std::vector<unsigned long long> desc;
   uint32_t ticket[4] = {0, 0, 0, 0};

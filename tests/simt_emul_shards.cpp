@@ -7,7 +7,7 @@
 //     the rank's base, give the oracle's minify of the whole buffer, cut at arbitrary bytes -- just after a backslash,
 //     inside strings, inside UTF-8 characters;
 //   - utf8v2's record for valid and corrupted shards cut at character boundaries.
-// The fold of the records (sjb200_capi.cu) is host code and is not run here.  Test infrastructure only.
+// The fold of the records (sjb200_comm.cu) is host code and is not run here.  Test infrastructure only.
 //
 // build: see tests/test_simt_emul_shards.py
 #define SJB200_HOST_EMU 1
@@ -115,7 +115,7 @@ int g_fail = 0;
     }                                                           \
   } while (0)
 
-// One launch over a whole shard, like sharded_enqueue / minify_shard_from: kind 0 stage 1, 1 minify, 2 validate_utf8.
+// One launch over a whole shard, like sharded_enqueue / scan_from_state: kind 0 stage 1, 1 minify, 2 validate_utf8.
 // nranks > 0: the last CTA stores the record for (seq, rank) into every window.  Returns the launch's carry out.
 Carry launch_shard(EmuJob &J, int kind, const uint8_t *buf, size_t len, uint32_t state_in, uint32_t *idx, uint8_t *dst, unsigned grid,
                    uint32_t nranks, uint32_t rank, uint32_t seq) {
@@ -132,8 +132,8 @@ Carry launch_shard(EmuJob &J, int kind, const uint8_t *buf, size_t len, uint32_t
   J.carry[1] = Carry();
   p.carry_in = state_in ? &J.carry[0] : nullptr;
   p.carry_out = &J.carry[1];
-  for (uint32_t r = 0; r < nranks; r++) p.xchg_peer[r] = J.window[r].data();
-  p.xchg_nranks = nranks; p.xchg_rank = rank; p.xchg_slot = (seq % uint32_t(kXchgSteps)) * 2u; p.xchg_seq = seq;
+  for (uint32_t r = 0; r < nranks; r++) p.xchg.peer[r] = J.window[r].data();
+  p.xchg.nranks = nranks; p.xchg.rank = rank; p.xchg.slot = (seq % uint32_t(kXchgSteps)) * 2u; p.xchg.seq = seq;
   unsigned g = grid;
   if (kind == kUtf8) {
     emu_launch(g, tmap, p, 3);
