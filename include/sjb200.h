@@ -53,6 +53,10 @@ enum {
   SJB200_UNESCAPED_CHARS = 14,
   SJB200_UNCLOSED_STRING = 15,
   SJB200_UNSUPPORTED_ARCHITECTURE = 16,
+  SJB200_INCORRECT_TYPE = 17,
+  SJB200_INDEX_OUT_OF_BOUNDS = 19,
+  SJB200_NO_SUCH_FIELD = 20,
+  SJB200_INVALID_JSON_POINTER = 22,
   SJB200_UNEXPECTED_ERROR = 24
 };
 
@@ -187,6 +191,39 @@ typedef struct {
 SJB200_API size_t sjb200_string_buf_capacity(size_t len);
 SJB200_API int sjb200_tokens_dev(sjb200_ctx *ctx, const uint8_t *d_buf, size_t len, const uint32_t *d_idx, uint32_t n, uint8_t *d_type, uint64_t *d_payload,
                       uint8_t *d_strbuf, size_t strbuf_capacity, sjb200_tokens_result *out, void *stream);
+
+/* JSON Pointer lookup on the device for every document of a stream: dom::element::at_pointer
+ * (include/simdjson/dom/element-inl.h L410-446, object-inl.h L104-147, array-inl.h L94-121, jsonpathutil.h L20-50) of
+ * every pointer in every document, batched, over the output of sjb200_tokens_dev (d_type, d_payload for n structurals,
+ * and its string buffer d_strbuf, of which string_bytes are in use).  d_docs / ndocs: a table from
+ * sjb200_document_table_dev; NULL or 0 = one document, structurals [0, n).  Document d is structurals
+ * [d_docs[d].index, d_docs[d + 1].index) (the last one: up to n).  pointers / pointer_lens: host strings (not
+ * NUL-terminated).  d_out: device memory, npointers x ndocs results (1 per pointer without a table), pointer-major:
+ * d_out[p * ndocs + d].  The results stay on the device; the call synchronises its stream once before it returns.
+ *
+ * A result is {SUCCESS, structural index of the selected value} -- d_type / d_payload / d_idx at that index give its
+ * type, its value or string-record offset, and its byte offset (a 'd' value is the span of its number, as for
+ * sjb200_tokens_dev) -- or {error, 0xFFFFFFFF} with the error at_pointer returns: INCORRECT_TYPE, INDEX_OUT_OF_BOUNDS,
+ * NO_SUCH_FIELD or INVALID_JSON_POINTER, in the reference's order of decision.  Two errors come first:
+ *   - a table entry that is not above the one before it, or not below n: UNEXPECTED_ERROR for that document;
+ *   - a token in error (d_type 0) in the document: {its d_payload error code, its structural index}, for the first such
+ *     token -- what dom::parser::parse reports for a document whose grammar is otherwise valid.
+ * Deviations from the reference: documents that parse rejects for their nesting get an error or an index inside the
+ * document, never a fault; max_depth is not enforced; root scalars are judged as sjb200_tokens_dev judges them; the walk
+ * follows the DOM API, not On-Demand.  A walk never reads outside [0, n) of the token arrays or [0, string_bytes) of the
+ * string buffer.
+ * Returns SUCCESS; CAPACITY, before any launch, beyond one of the limits below; MEMALLOC or UNEXPECTED_ERROR for a CUDA
+ * failure or bad arguments. */
+#define SJB200_POINTER_MAX_POINTERS 65536   /* pointers per call */
+#define SJB200_POINTER_MAX_TOKENS 1024      /* reference tokens per pointer */
+#define SJB200_POINTER_MAX_BYTES 1048576    /* bytes of all pointers of a call */
+typedef struct {
+  int32_t error;
+  uint32_t index;
+} sjb200_pointer_result;
+SJB200_API int sjb200_at_pointer_dev(sjb200_ctx *ctx, const uint8_t *d_type, const uint64_t *d_payload, uint32_t n, const uint8_t *d_strbuf,
+                                     size_t string_bytes, const sjb200_doc_boundary *d_docs, uint32_t ndocs, const char *const *pointers,
+                                     const size_t *pointer_lens, int npointers, sjb200_pointer_result *d_out, void *stream);
 
 /* split form of the same calls for pipelining / timing: enqueue returns as soon as the work is on the
  * stream, finish waits for it and completes the reference's finish() logic. */

@@ -14,6 +14,7 @@
 #include "sjb200_finish.h"
 #include "sjb200_hostpipe.h"
 #include "sjb200_kernels.cuh"
+#include "sjb200_pointer.h"
 
 using namespace sjb200;
 
@@ -296,6 +297,8 @@ extern "C" void sjb200_destroy(sjb200_ctx *c) {
   if (c->stream) cudaStreamSynchronize(c->stream);
   free_sized(c);
   cudaFree(c->d_carry); cudaFree(c->d_flags); cudaFree(c->d_ticket); cudaFree(c->d_sfin); cudaFree(c->d_doc_scratch); cudaFree(c->d_ndocs); cudaFree(c->d_tok_scratch); cudaFree(c->d_tok_tot); cudaFree(c->d_tails); cudaFree(c->d_debug); cudaFree(c->d_doctab); cudaFree(c->d_stamps);
+  cudaFree(c->d_ptr_blob); cudaFree(c->d_ptr_scratch);
+  if (c->h_ptr_blob) cudaFreeHost(c->h_ptr_blob);
   if (c->h_doctab) cudaFreeHost(c->h_doctab);
   if (c->h_carry) cudaFreeHost(c->h_carry);
   if (c->h_flags) cudaFreeHost(c->h_flags);
@@ -796,6 +799,55 @@ extern "C" int sjb200_tokens_dev(sjb200_ctx *c, const uint8_t *d_buf, size_t len
     out->error = SJB200_CAPACITY;
   }
   return out->error;
+}
+
+// JSON Pointer lookup over the stage-2-lite tokens (dom::element::at_pointer for every document and pointer) --
+// sjb200_pointer.cu
+extern "C" int sjb200_at_pointer_dev(sjb200_ctx *c, const uint8_t *d_type, const uint64_t *d_payload, uint32_t n, const uint8_t *d_strbuf,
+                                     size_t string_bytes, const sjb200_doc_boundary *d_docs, uint32_t ndocs, const char *const *pointers,
+                                     const size_t *pointer_lens, int npointers, sjb200_pointer_result *d_out, void *stream) {
+  if (!c || npointers < 0 || (npointers && (!pointers || !pointer_lens || !d_out)) || (n && (!d_type || !d_payload)) ||
+      (string_bytes && !d_strbuf))
+    return SJB200_UNEXPECTED_ERROR;
+  static_assert(sizeof(sjb200_pointer_result) == sizeof(ptr::PtrResult), "layout");
+  ptr::CompiledPointers cp;
+  const int rc = ptr::compile_pointers(pointers, pointer_lens, npointers, &cp);
+  if (rc != SJB200_SUCCESS) return rc;
+  if (npointers == 0) return SJB200_SUCCESS;
+  if (!d_docs) ndocs = 0;
+  DeviceGuard g(c->device);
+  cudaStream_t s = stream_of(c, stream);
+  // one blob [headers][levels][keys], copied in one transfer from pinned memory
+  const size_t hb = cp.headers.size() * sizeof(ptr::PtrHeader), lb = cp.levels.size() * sizeof(ptr::PtrLevel);
+  const size_t need = hb + lb + cp.keys.size() + 1;
+  if (c->ptr_blob_bytes < need) {
+    if (c->h_ptr_blob) cudaFreeHost(c->h_ptr_blob);
+    c->h_ptr_blob = nullptr;
+    c->ptr_blob_bytes = 0;
+    cudaFree(c->d_ptr_blob);
+    c->d_ptr_blob = nullptr;
+    if (!ok(c, cudaMallocHost(&c->h_ptr_blob, need), "cudaMallocHost(pointers)") || !dev_alloc(c, &c->d_ptr_blob, need, "cudaMalloc(pointers)"))
+      return SJB200_MEMALLOC;
+    c->ptr_blob_bytes = need;
+  }
+  memcpy(c->h_ptr_blob, cp.headers.data(), hb);
+  memcpy(c->h_ptr_blob + hb, cp.levels.data(), lb);
+  memcpy(c->h_ptr_blob + hb + lb, cp.keys.data(), cp.keys.size());
+  if (!grow(c, &c->d_ptr_scratch, &c->ptr_scratch_words, ptr::pointer_scratch_words(ndocs ? ndocs : 1), "cudaMalloc(pointer scratch)"))
+    return SJB200_MEMALLOC;
+  ptr::PtrLaunch a{};
+  a.w = ptr::Walk{d_type, d_payload, d_strbuf, string_bytes, reinterpret_cast<const ptr::PtrLevel *>(c->d_ptr_blob + hb), c->d_ptr_blob + hb + lb};
+  a.n = n;
+  a.docs = ndocs ? reinterpret_cast<const sjb200_doc_boundary_t *>(d_docs) : nullptr;
+  a.ndocs = ndocs;
+  a.headers = reinterpret_cast<const ptr::PtrHeader *>(c->d_ptr_blob);
+  a.npointers = uint32_t(npointers);
+  a.out = reinterpret_cast<ptr::PtrResult *>(d_out);
+  if (!ok(c, cudaMemcpyAsync(c->d_ptr_blob, c->h_ptr_blob, need, cudaMemcpyHostToDevice, s), "H2D pointers") ||
+      !ok(c, ptr::launch_at_pointer(a, c->d_ptr_scratch, c->sm_count, s), "at_pointer") || !ok(c, cudaStreamSynchronize(s), "sync"))
+    return SJB200_UNEXPECTED_ERROR;
+  c->launches += 3;
+  return SJB200_SUCCESS;
 }
 
 extern "C" int sjb200_stage1_dev(sjb200_ctx *c, const uint8_t *d_buf, size_t len, int mode, uint32_t *d_idx, uint32_t *n_inout,

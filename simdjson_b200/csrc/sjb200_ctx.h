@@ -69,6 +69,9 @@ struct sjb200_ctx {
   sjb200::StreamFinish *d_sfin = nullptr;  // [kCarrySlots] results of the device-side streaming epilogue
   uint32_t *d_doc_scratch = nullptr; size_t doc_scratch_words = 0; uint32_t *d_ndocs = nullptr;
   uint8_t *d_tok_scratch = nullptr; size_t tok_scratch_bytes = 0; sjb200::TokenTotals *d_tok_tot = nullptr;  // stage-2-lite (sjb200_tape.cu)
+  // JSON Pointer lookup (sjb200_pointer.cu): the compiled pointers, pinned and on the device (ptr_blob_bytes each), scratch
+  uint8_t *h_ptr_blob = nullptr; uint8_t *d_ptr_blob = nullptr; size_t ptr_blob_bytes = 0;
+  uint32_t *d_ptr_scratch = nullptr; size_t ptr_scratch_words = 0;
   int grid_u = 0;
   // pinned host mirrors
   sjb200::Carry *h_carry = nullptr;     // [kCarrySlots]

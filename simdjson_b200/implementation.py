@@ -190,6 +190,30 @@ class dom_parser_implementation:
                                 d_strbuf.data_ptr() if cap else None, cap, C.byref(res), _stream_ptr(stream))
         return res, d_type[:n], d_payload[:n], d_strbuf
 
+    def at_pointer_device(self, pointers, d_type, d_payload, d_strbuf, string_bytes, d_docs=None, ndocs=None, stream=None):
+        """dom::element::at_pointer of every pointer (str or bytes) in every document, on the device (sjb200_at_pointer_dev)
+        over the output of tokens_device: d_docs = a document table (sjb200_document_table_dev, int32 pairs
+        {index, byte}) and ndocs its entries in use, or None for one document.  Returns (error int32[P, D], index
+        int32[P, D]) CUDA tensors: the index is the structural index of the selected value (0xFFFFFFFF, i.e. -1, on an
+        error other than a token error).  A failure of the call itself raises."""
+        import torch
+        enc = [p.encode() if isinstance(p, str) else bytes(p) for p in pointers]
+        P = len(enc)
+        D = 1 if d_docs is None else (d_docs.numel() * d_docs.element_size() // 8 if ndocs is None else int(ndocs))
+        dev = d_type.device
+        out = torch.empty((P, max(D, 1), 2), dtype=torch.int32, device=dev)
+        bufs = [C.create_string_buffer(e, len(e)) for e in enc]
+        ptrs = (C.c_void_p * max(P, 1))(*[C.addressof(b) for b in bufs])
+        lens = (C.c_size_t * max(P, 1))(*[len(e) for e in enc])
+        n = d_type.numel()
+        rc = lib().sjb200_at_pointer_dev(self._ctx, d_type.data_ptr() if n else None, d_payload.data_ptr() if n else None, n,
+                                         d_strbuf.data_ptr() if string_bytes else None, string_bytes,
+                                         None if d_docs is None else d_docs.data_ptr(), 0 if d_docs is None else D, ptrs, lens, P,
+                                         out.data_ptr() if P else None, _stream_ptr(stream))
+        if rc != SUCCESS:
+            raise RuntimeError(f"sjb200_at_pointer_dev: {capi.ERROR_NAMES.get(rc, rc)} {self.last_cuda_error()}")
+        return out[:, :D, 0], out[:, :D, 1]
+
     def stage1_shard_device(self, d_buf, state_in=0, last_shard=True, d_idx=None, stream=None):
         """one GPU's piece of a sharded scan; returns (error_code, capi.ShardResult)"""
         if d_idx is None:
