@@ -1,6 +1,7 @@
 // b200_implementation.cpp -- see b200_implementation.h
 #include "b200_implementation.h"
 
+#include <atomic>
 #include <cstdlib>
 #include <cstring>
 #include <mutex>
@@ -31,7 +32,11 @@ struct thread_context {
 };
 thread_local thread_context tls_context;
 
+std::atomic<uint64_t> total_gpu_calls{0};
+
 }  // namespace
+
+uint64_t gpu_stage1_calls_total() noexcept { return total_gpu_calls.load(); }
 
 // ---------------------------------------------------------------- implementation
 error_code implementation::create_dom_parser_implementation(size_t capacity, size_t max_depth,
@@ -122,6 +127,7 @@ error_code dom_parser_implementation::stage1(const uint8_t *buf, size_t len, sta
   len_ = len;  // the reference keeps the untrimmed length here too (src/icelake.cpp L179-181)
   if (!ctx_) return UNINITIALIZED;
   gpu_calls_++;
+  total_gpu_calls++;
   const int rc = sjb200_stage1(ctx_, buf, len, int(mode), structural_indexes.get(), &n_structural_indexes);
   // next_structural_index = 0 is stored together with the sentinels (json_structural_indexer.h L284-287),
   // i.e. on every path that got past the early returns

@@ -78,6 +78,10 @@ class dom_parser_implementation final : public internal::dom_parser_implementati
 // the singleton to assign to simdjson::get_active_implementation()
 const implementation *get_implementation(int device = 0) noexcept;
 
+// stage-1 calls sent to the GPU by every parser of this process so far (the On-Demand parser keeps its
+// implementation private, and a threaded document_stream swaps two parsers: tests count through this)
+uint64_t gpu_stage1_calls_total() noexcept;
+
 }  // namespace b200
 }  // namespace simdjson
 
