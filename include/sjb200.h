@@ -209,7 +209,8 @@ SJB200_API int sjb200_tokens_dev(sjb200_ctx *ctx, const uint8_t *d_buf, size_t l
  *   - a token in error (d_type 0) in the document: {its d_payload error code, its structural index}, for the first such
  *     token -- what dom::parser::parse reports for a document whose grammar is otherwise valid.
  * Deviations from the reference: documents that parse rejects for their nesting get an error or an index inside the
- * document, never a fault; max_depth is not enforced; root scalars are judged as sjb200_tokens_dev judges them; the walk
+ * document, never a fault (sjb200_document_errors_dev gives the exact parse error: drop the results of the documents
+ * whose verdict there is not SUCCESS); max_depth is not enforced; root scalars are judged as sjb200_tokens_dev judges them; the walk
  * follows the DOM API, not On-Demand.  A walk never reads outside [0, n) of the token arrays or [0, string_bytes) of the
  * string buffer.
  * Returns SUCCESS; CAPACITY, before any launch, beyond one of the limits below; MEMALLOC or UNEXPECTED_ERROR for a CUDA
@@ -224,6 +225,35 @@ typedef struct {
 SJB200_API int sjb200_at_pointer_dev(sjb200_ctx *ctx, const uint8_t *d_type, const uint64_t *d_payload, uint32_t n, const uint8_t *d_strbuf,
                                      size_t string_bytes, const sjb200_doc_boundary *d_docs, uint32_t ndocs, const char *const *pointers,
                                      const size_t *pointer_lens, int npointers, sjb200_pointer_result *d_out, void *stream);
+
+/* Stage-2 grammar on the device: for every document, the error json_iterator::walk_document
+ * (src/generic/stage2/json_iterator.h L120-244, with tape_builder) returns, from the output of sjb200_tokens_dev (d_type,
+ * d_payload for n structurals of a regular-mode stage 1 that succeeded).  No table (d_docs NULL or ndocs 0): one document
+ * [0, n), as dom::parser::parse judges it (n = 0: {EMPTY, 0}).  With a table from sjb200_document_table_dev: document d
+ * is [d_docs[d].index, d_docs[d + 1].index) (the last one: up to n), as stage2_next from its first structural judges it
+ * (document_stream-inl.h L250-269); a walk that ends before the document's end is a TAPE_ERROR at the first structural
+ * left over, one that would read the structural at the end a TAPE_ERROR at the end.
+ * d_out (device memory, one per document): {error, structural index at which it was decided}, or {SUCCESS, one past the
+ * document's value}.  *out: the documents in error and the first of them.  One stream synchronise.  A caller of
+ * sjb200_at_pointer_dev gets the exact parse error by dropping the results of documents whose verdict is not SUCCESS.
+ * Deviations: an infinite float (1e400) is SUCCESS (the tokens check only float grammar); a root token starting with a
+ * byte below '0' other than '-' (+1, #) is NUMBER_ERROR, not TAPE_ERROR (the tokens do not keep the byte); the last
+ * document of a stream that wants a value past n is a TAPE_ERROR at n (the reference judges its padding byte there).
+ * Returns SUCCESS; CAPACITY, before any launch and with nothing written, for max_depth 0 or above
+ * SJB200_DOCUMENT_MAX_DEPTH; UNEXPECTED_ERROR when the table is not strictly ascending or has an entry at or above n
+ * (every result {UNEXPECTED_ERROR, 0xFFFFFFFF}); MEMALLOC or UNEXPECTED_ERROR for a CUDA failure or bad arguments. */
+#define SJB200_DOCUMENT_MAX_DEPTH 4096
+typedef struct {
+  int32_t error;   /* simdjson::error_code */
+  uint32_t index;  /* structural index at which it was decided; SUCCESS: one past the document's value */
+} sjb200_document_error;
+typedef struct {
+  uint32_t ndocs_in_error;
+  uint32_t first_doc_in_error;  /* 0xFFFFFFFF when none: where parse_many stops */
+} sjb200_document_errors_result;
+SJB200_API int sjb200_document_errors_dev(sjb200_ctx *ctx, const uint8_t *d_type, const uint64_t *d_payload, uint32_t n,
+                                          const sjb200_doc_boundary *d_docs, uint32_t ndocs, size_t max_depth,
+                                          sjb200_document_error *d_out, sjb200_document_errors_result *out, void *stream);
 
 /* split form of the same calls for pipelining / timing: enqueue returns as soon as the work is on the
  * stream, finish waits for it and completes the reference's finish() logic. */

@@ -28,17 +28,20 @@ EXPORTS = [
     "sjb200_document_table_shard_dev", "sjb200_stream_fold",
     "sjb200_stage1_sharded_delimited", "sjb200_stage1_sharded_delimited_enqueue", "sjb200_stage1_sharded_delimited_finish", "sjb200_delimited_fold",
     "sjb200_tokens_sharded", "sjb200_tokens_sharded_enqueue", "sjb200_tokens_sharded_finish",
-    "sjb200_at_pointer_dev",
+    "sjb200_at_pointer_dev", "sjb200_document_errors_dev",
 ]
 COMM_HANDLE_BYTES = 64
 
 # simdjson::error_code values of this path (include/simdjson/error.h L19-54)
 SUCCESS, CAPACITY, MEMALLOC, UTF8_ERROR, EMPTY, UNESCAPED_CHARS, UNCLOSED_STRING, UNSUPPORTED_ARCHITECTURE, UNEXPECTED_ERROR = 0, 1, 2, 11, 13, 14, 15, 16, 24
-ERROR_NAMES = {0: "SUCCESS", 1: "CAPACITY", 2: "MEMALLOC", 3: "TAPE_ERROR", 5: "STRING_ERROR", 6: "T_ATOM_ERROR", 7: "F_ATOM_ERROR", 8: "N_ATOM_ERROR",
+ERROR_NAMES = {0: "SUCCESS", 1: "CAPACITY", 2: "MEMALLOC", 3: "TAPE_ERROR", 4: "DEPTH_ERROR", 5: "STRING_ERROR", 6: "T_ATOM_ERROR", 7: "F_ATOM_ERROR", 8: "N_ATOM_ERROR",
                9: "NUMBER_ERROR", 10: "BIGINT_ERROR", 11: "UTF8_ERROR", 13: "EMPTY", 14: "UNESCAPED_CHARS", 15: "UNCLOSED_STRING",
                16: "UNSUPPORTED_ARCHITECTURE", 17: "INCORRECT_TYPE", 19: "INDEX_OUT_OF_BOUNDS", 20: "NO_SUCH_FIELD", 22: "INVALID_JSON_POINTER",
                24: "UNEXPECTED_ERROR"}
 INCORRECT_TYPE, INDEX_OUT_OF_BOUNDS, NO_SUCH_FIELD, INVALID_JSON_POINTER = 17, 19, 20, 22
+DEPTH_ERROR = 4
+# the deepest max_depth sjb200_document_errors_dev accepts (SJB200_DOCUMENT_MAX_DEPTH)
+DOCUMENT_MAX_DEPTH = 4096
 # limits of sjb200_at_pointer_dev (SJB200_POINTER_MAX_*)
 POINTER_MAX_POINTERS, POINTER_MAX_TOKENS, POINTER_MAX_BYTES = 65536, 1024, 1 << 20
 
@@ -114,6 +117,10 @@ class PointerResult(C.Structure):
     _fields_ = [("error", C.c_int32), ("index", C.c_uint32)]
 
 
+class DocumentErrorsResult(C.Structure):
+    _fields_ = [("ndocs_in_error", C.c_uint32), ("first_doc_in_error", C.c_uint32)]
+
+
 def load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
@@ -185,6 +192,7 @@ def load():
         "sjb200_tokens_sharded_enqueue": (C.c_int, [vp, vp, sz, C.c_uint32, vp, C.c_uint32, vp, vp, vp, sz, vp]),
         "sjb200_tokens_sharded_finish": (C.c_int, [vp, C.POINTER(ShardedTokensResult)]),
         "sjb200_at_pointer_dev": (C.c_int, [vp, vp, vp, C.c_uint32, vp, sz, vp, C.c_uint32, vp, vp, C.c_int, vp, vp]),
+        "sjb200_document_errors_dev": (C.c_int, [vp, vp, vp, C.c_uint32, vp, C.c_uint32, sz, vp, C.POINTER(DocumentErrorsResult), vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)

@@ -14,6 +14,7 @@
 #include "sjb200_finish.h"
 #include "sjb200_hostpipe.h"
 #include "sjb200_kernels.cuh"
+#include "sjb200_grammar.h"
 #include "sjb200_pointer.h"
 
 using namespace sjb200;
@@ -297,7 +298,7 @@ extern "C" void sjb200_destroy(sjb200_ctx *c) {
   if (c->stream) cudaStreamSynchronize(c->stream);
   free_sized(c);
   cudaFree(c->d_carry); cudaFree(c->d_flags); cudaFree(c->d_ticket); cudaFree(c->d_sfin); cudaFree(c->d_doc_scratch); cudaFree(c->d_ndocs); cudaFree(c->d_tok_scratch); cudaFree(c->d_tok_tot); cudaFree(c->d_tails); cudaFree(c->d_debug); cudaFree(c->d_doctab); cudaFree(c->d_stamps);
-  cudaFree(c->d_ptr_blob); cudaFree(c->d_ptr_scratch);
+  cudaFree(c->d_ptr_blob); cudaFree(c->d_ptr_scratch); cudaFree(c->d_gram_scratch);
   if (c->h_ptr_blob) cudaFreeHost(c->h_ptr_blob);
   if (c->h_doctab) cudaFreeHost(c->h_doctab);
   if (c->h_carry) cudaFreeHost(c->h_carry);
@@ -848,6 +849,41 @@ extern "C" int sjb200_at_pointer_dev(sjb200_ctx *c, const uint8_t *d_type, const
     return SJB200_UNEXPECTED_ERROR;
   c->launches += 3;
   return SJB200_SUCCESS;
+}
+
+// Stage-2 grammar over the stage-2-lite tokens (the error walk_document returns for every document) -- sjb200_grammar.cu
+extern "C" int sjb200_document_errors_dev(sjb200_ctx *c, const uint8_t *d_type, const uint64_t *d_payload, uint32_t n, const sjb200_doc_boundary *d_docs,
+                                          uint32_t ndocs, size_t max_depth, sjb200_document_error *d_out, sjb200_document_errors_result *out,
+                                          void *stream) {
+  if (!c || !d_out || !out || (n && (!d_type || !d_payload))) return SJB200_UNEXPECTED_ERROR;
+  if (max_depth == 0 || max_depth > SJB200_DOCUMENT_MAX_DEPTH) return SJB200_CAPACITY;
+  static_assert(sizeof(sjb200_document_error) == sizeof(gram::DocError), "layout");
+  static_assert(SJB200_DOCUMENT_MAX_DEPTH == gram::kMaxDepth, "limit");
+  if (!d_docs) ndocs = 0;
+  DeviceGuard g(c->device);
+  cudaStream_t s = stream_of(c, stream);
+  const size_t words = gram::grammar_scratch_words(n, ndocs, uint32_t(max_depth));
+  if (!grow(c, &c->d_gram_scratch, &c->gram_scratch_words, words + 4, "cudaMalloc(grammar scratch)")) return SJB200_MEMALLOC;
+  gram::GrammarArgs a{};
+  a.type = d_type;
+  a.payload = d_payload;
+  a.n = n;
+  a.docs = ndocs ? reinterpret_cast<const sjb200_doc_boundary_t *>(d_docs) : nullptr;
+  a.ndocs = ndocs;
+  a.max_depth = uint32_t(max_depth);
+  a.out = reinterpret_cast<gram::DocError *>(d_out);
+  uint32_t *summary = c->d_gram_scratch + words;
+  int launched = 0;
+  if (!ok(c, gram::launch_document_errors(a, c->d_gram_scratch, summary, c->sm_count, s, &launched), "document_errors") ||
+      !ok(c, cudaMemcpyAsync(c->h_small, summary, 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s), "D2H summary") ||
+      !ok(c, cudaStreamSynchronize(s), "sync"))
+    return SJB200_UNEXPECTED_ERROR;
+  c->launches += unsigned(launched);
+  uint32_t sum[3];
+  memcpy(sum, c->h_small, sizeof(sum));
+  out->ndocs_in_error = sum[1];
+  out->first_doc_in_error = sum[2];
+  return sum[0] ? SJB200_UNEXPECTED_ERROR : SJB200_SUCCESS;
 }
 
 extern "C" int sjb200_stage1_dev(sjb200_ctx *c, const uint8_t *d_buf, size_t len, int mode, uint32_t *d_idx, uint32_t *n_inout,

@@ -72,6 +72,7 @@ struct sjb200_ctx {
   // JSON Pointer lookup (sjb200_pointer.cu): the compiled pointers, pinned and on the device (ptr_blob_bytes each), scratch
   uint8_t *h_ptr_blob = nullptr; uint8_t *d_ptr_blob = nullptr; size_t ptr_blob_bytes = 0;
   uint32_t *d_ptr_scratch = nullptr; size_t ptr_scratch_words = 0;
+  uint32_t *d_gram_scratch = nullptr; size_t gram_scratch_words = 0;  // stage-2 grammar (sjb200_grammar.cu)
   int grid_u = 0;
   // pinned host mirrors
   sjb200::Carry *h_carry = nullptr;     // [kCarrySlots]

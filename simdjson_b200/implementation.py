@@ -55,9 +55,10 @@ def _stream_ptr(stream):
 class dom_parser_implementation:
     """One parser instance = one CUDA context object (own stream and scratch)."""
 
-    def __init__(self, device=0):
+    def __init__(self, device=0, max_depth=1024):
         self._ctx = C.c_void_p()
         self._device = device
+        self.max_depth = max_depth  # the stage-2 depth limit (document_errors_device)
         self._capacity = 0
         self.n_structural_indexes = 0
         self.structural_indexes = None  # numpy uint32[ROUNDUP(capacity,64)+9] (host calls)
@@ -214,6 +215,24 @@ class dom_parser_implementation:
             raise RuntimeError(f"sjb200_at_pointer_dev: {capi.ERROR_NAMES.get(rc, rc)} {self.last_cuda_error()}")
         return out[:, :D, 0], out[:, :D, 1]
 
+    def document_errors_device(self, d_type, d_payload, d_docs=None, ndocs=None, max_depth=None, stream=None):
+        """the error stage 2 returns for every document (sjb200_document_errors_dev) over the output of tokens_device:
+        d_docs = a document table (sjb200_document_table_dev, int32 pairs {index, byte}) and ndocs its entries in use, or
+        None for one document; max_depth defaults to the parser's.  Returns (capi.DocumentErrorsResult, error int32[D],
+        index int32[D]) with the results on the device: the index is the structural at which the error was decided, one
+        past the document's value on SUCCESS (0xFFFFFFFF, i.e. -1, for a bad table).  A failure of the call raises."""
+        import torch
+        D = 1 if d_docs is None else (d_docs.numel() * d_docs.element_size() // 8 if ndocs is None else int(ndocs))
+        out = torch.empty((max(D, 1), 2), dtype=torch.int32, device=d_type.device)
+        res = capi.DocumentErrorsResult()
+        n = d_type.numel()
+        rc = lib().sjb200_document_errors_dev(self._ctx, d_type.data_ptr() if n else None, d_payload.data_ptr() if n else None, n,
+                                              None if d_docs is None else d_docs.data_ptr(), 0 if d_docs is None else D,
+                                              self.max_depth if max_depth is None else max_depth, out.data_ptr(), C.byref(res), _stream_ptr(stream))
+        if rc != SUCCESS:
+            raise RuntimeError(f"sjb200_document_errors_dev: {capi.ERROR_NAMES.get(rc, rc)} {self.last_cuda_error()}")
+        return res, out[:D, 0], out[:D, 1]
+
     def stage1_shard_device(self, d_buf, state_in=0, last_shard=True, d_idx=None, stream=None):
         """one GPU's piece of a sharded scan; returns (error_code, capi.ShardResult)"""
         if d_idx is None:
@@ -288,9 +307,8 @@ class implementation:
         return rc == SUCCESS
 
     def create_dom_parser_implementation(self, capacity, max_depth=1024):
-        """-> (error_code, parser or None); L97-101"""
-        _ = max_depth  # stage 2 stacks are not part of this path
-        p = dom_parser_implementation(self._device)
+        """-> (error_code, parser or None); L97-101.  max_depth is the default of document_errors_device."""
+        p = dom_parser_implementation(self._device, max_depth)
         rc = p._create(capacity)
         return (rc, p) if rc == SUCCESS else (rc, None)
 
