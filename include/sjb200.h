@@ -450,6 +450,49 @@ SJB200_API int sjb200_tokens_sharded(sjb200_comm *comm, const uint8_t *d_shard, 
                           uint8_t *d_type, uint64_t *d_payload, uint8_t *d_strbuf, size_t strbuf_capacity, sjb200_sharded_tokens_result *out,
                           void *stream);
 
+/* stage-2 grammar (sjb200_document_errors_dev) sharded the same way, on the same comm and window: every rank judges its
+ * own structurals, and three host-synchronised rounds carry what crosses the cuts -- the edges (each rank's n, table and
+ * the types of its first two and last two structurals), the stack records (the containers open at each rank's end) and
+ * the results (each rank's first error before its first document start, and its counts).  A grammar pass has its own
+ * kind.  (d_type, d_payload, n) is this rank's output of sjb200_tokens_sharded; n may be 0.
+ *   whole = 1: the ranks together hold ONE document, judged as dom::parser::parse judges it; d_docs / ndocs are ignored.
+ *   whole = 0: d_docs / ndocs is this rank's table from sjb200_document_table_shard_dev (ndocs may be 0: a rank inside
+ *              one long document).
+ * Every rank passes the same whole and max_depth.  The contract: gather the inputs -- the concatenations of the ranks'
+ * types, payloads, and tables with index + tokens_before -- and run sjb200_document_errors_dev on them.  Rank r writes
+ * d_out[j] for the j-th document that STARTS on it (whole mode: rank 0 writes the one result), each {error, 64-bit
+ * global structural index}; concatenated over the ranks they equal that call's d_out (whose 0xFFFFFFFF is UINT64_MAX
+ * here).  The stream's structural 0 starts a segment whatever its rank's table says, as bit 0 does there.  One exception:
+ * whole = 0 with no document on any rank writes nothing, reports 0 documents and returns SUCCESS.
+ * finish returns, on every rank alike, the error code of that call: CAPACITY (nothing written) when a rank's max_depth
+ * is 0 or above SJB200_DOCUMENT_MAX_DEPTH; UNEXPECTED_ERROR when any rank's table is bad (every result then
+ * {UNEXPECTED_ERROR, UINT64_MAX}), when the ranks disagree on whole or max_depth, when a peer enqueued another kind for
+ * the pass, or when a rank could not run its pass; else SUCCESS.  Deviations, as for sjb200_document_errors_dev: an
+ * infinite float (1e400) is SUCCESS; a root token starting with a byte below '0' other than '-' (+1, #) is NUMBER_ERROR;
+ * the last document wanting a value past the stream's end is a TAPE_ERROR at the global n. */
+typedef struct {
+  int32_t error;     /* simdjson::error_code */
+  uint32_t reserved;
+  uint64_t index;    /* global structural index at which it was decided (SUCCESS: one past the document's value); UINT64_MAX: none */
+} sjb200_sharded_document_error;
+typedef struct {
+  int error;                    /* as returned */
+  int32_t first_error;          /* the error of first_doc_in_error (SUCCESS when none) */
+  uint64_t docs_before;         /* documents starting on earlier ranks: d_out[j] here is document docs_before + j */
+  uint64_t tokens_before;       /* structurals of earlier ranks */
+  uint64_t ndocs;               /* documents of the stream */
+  uint64_t ndocs_in_error;
+  uint64_t first_doc_in_error;  /* global document number; UINT64_MAX when none */
+  uint64_t first_error_index;   /* its global structural index; UINT64_MAX when none */
+} sjb200_sharded_document_errors_result;
+SJB200_API int sjb200_document_errors_sharded_enqueue(sjb200_comm *comm, const uint8_t *d_type, const uint64_t *d_payload, uint32_t n, int whole,
+                                                      const sjb200_doc_boundary *d_docs, uint32_t ndocs, size_t max_depth,
+                                                      sjb200_sharded_document_error *d_out, void *stream);
+SJB200_API int sjb200_document_errors_sharded_finish(sjb200_comm *comm, sjb200_sharded_document_errors_result *out);
+SJB200_API int sjb200_document_errors_sharded(sjb200_comm *comm, const uint8_t *d_type, const uint64_t *d_payload, uint32_t n, int whole,
+                                              const sjb200_doc_boundary *d_docs, uint32_t ndocs, size_t max_depth,
+                                              sjb200_sharded_document_error *d_out, sjb200_sharded_document_errors_result *out, void *stream);
+
 /* the document starts of one shard of a sharded stream pass: (local structural index, shard-relative byte) pairs of
  * d_idx[0, kept), structural 0 counted when first_starts_document says so (both from the pass's result).  A rank's
  * global document numbers are its table's positions plus the other ranks' ndocs before it.  Not collective.
@@ -523,6 +566,48 @@ typedef struct {
 } sjb200_delimited_fold_result;
 SJB200_API int sjb200_delimited_fold(int mode, int nranks, uint32_t final_state, uint32_t flags_all, const sjb200_delimited_summary *sums,
                           sjb200_delimited_fold_result *res, sjb200_delimited_rank *ranks /* nranks */);
+
+/* the host folds of a sharded grammar pass, pure: what every rank's finish computes.  The edge round, per rank: */
+typedef struct {
+  uint32_t n;            /* structurals */
+  uint32_t ndocs;        /* table entries (whole mode: 0) */
+  uint32_t flags;        /* bit0 the rank could not run its pass, bit1 bad table, bit2 whole, bit3 the table starts at 0,
+                            bit4 its last entry is n - 1 */
+  uint32_t max_depth;
+  uint32_t types;        /* types of structurals 0, 1, n - 2, n - 1, a byte each from the low one (0xFF: none) */
+  uint32_t first_start;  /* the table's first entry (ndocs > 0) */
+} sjb200_grammar_edge;
+typedef struct {
+  uint64_t tokens_before;
+  uint64_t docs_before;
+  uint32_t owned;        /* documents that start on this rank (whole mode: 1 on rank 0) */
+  uint32_t holds_root;   /* this rank's structural 0 is the stream's */
+  uint32_t halo_before;  /* types of the two structurals before this rank's 0: byte 0 the earlier one (0xFF: none) */
+  uint32_t halo_after;   /* type of the structural after this rank's last (0xFF: none) */
+  uint32_t halo_flags;   /* bit0 the structural before this rank's 0 starts a document, bit1 the one after its last does,
+                            bit2 holds_root */
+  uint32_t last_type;    /* type of the stream's last structural (0xFF: none) */
+} sjb200_grammar_rank;
+typedef struct {
+  int error;             /* SUCCESS, CAPACITY or UNEXPECTED_ERROR (a failed rank, whole / max_depth disagree) */
+  uint32_t bad_table;    /* some rank's table is bad */
+  uint64_t n;            /* structurals of the stream */
+  uint64_t ndocs;        /* documents of the stream */
+} sjb200_grammar_edge_fold_result;
+SJB200_API int sjb200_grammar_edge_fold(int nranks, const sjb200_grammar_edge *edges, sjb200_grammar_edge_fold_result *res,
+                                        sjb200_grammar_rank *ranks /* nranks */);
+/* the result round, per rank: errors as keys global index << 8 | code (UINT64_MAX: none) */
+typedef struct {
+  uint64_t lead;         /* the first error among its structurals before its first document start */
+  uint64_t last;         /* the first error its own structurals give its last document */
+  uint64_t first_key;    /* that of first_doc */
+  uint32_t errors;       /* its documents in error, the last one left out */
+  uint32_t first_doc;    /* the first of them (0xFFFFFFFF: none) */
+} sjb200_grammar_tally;
+/* fills out's error, first_error, ndocs, ndocs_in_error, first_doc_in_error, first_error_index, and last[r], the result
+ * of rank r's last document (ranks that own none: unchanged).  Returns out->error. */
+SJB200_API int sjb200_grammar_result_fold(int nranks, const sjb200_grammar_edge *edges, const sjb200_grammar_tally *tallies,
+                                          sjb200_sharded_document_errors_result *out, sjb200_sharded_document_error *last /* nranks */);
 
 /* fold: state entering shard r given the ttables of shards 0..r-1 and the document's initial state 0 */
 SJB200_API uint32_t sjb200_fold_state(const uint32_t *ttables, int nshards_before);

@@ -29,6 +29,8 @@ EXPORTS = [
     "sjb200_stage1_sharded_delimited", "sjb200_stage1_sharded_delimited_enqueue", "sjb200_stage1_sharded_delimited_finish", "sjb200_delimited_fold",
     "sjb200_tokens_sharded", "sjb200_tokens_sharded_enqueue", "sjb200_tokens_sharded_finish",
     "sjb200_at_pointer_dev", "sjb200_document_errors_dev",
+    "sjb200_document_errors_sharded", "sjb200_document_errors_sharded_enqueue", "sjb200_document_errors_sharded_finish",
+    "sjb200_grammar_edge_fold", "sjb200_grammar_result_fold",
 ]
 COMM_HANDLE_BYTES = 64
 
@@ -121,6 +123,32 @@ class DocumentErrorsResult(C.Structure):
     _fields_ = [("ndocs_in_error", C.c_uint32), ("first_doc_in_error", C.c_uint32)]
 
 
+class ShardedDocumentError(C.Structure):
+    _fields_ = [("error", C.c_int32), ("reserved", C.c_uint32), ("index", C.c_uint64)]
+
+
+class ShardedDocumentErrorsResult(C.Structure):
+    _fields_ = [("error", C.c_int), ("first_error", C.c_int32), ("docs_before", C.c_uint64), ("tokens_before", C.c_uint64), ("ndocs", C.c_uint64),
+                ("ndocs_in_error", C.c_uint64), ("first_doc_in_error", C.c_uint64), ("first_error_index", C.c_uint64)]
+
+
+class GrammarEdge(C.Structure):
+    _fields_ = [("n", C.c_uint32), ("ndocs", C.c_uint32), ("flags", C.c_uint32), ("max_depth", C.c_uint32), ("types", C.c_uint32), ("first_start", C.c_uint32)]
+
+
+class GrammarRank(C.Structure):
+    _fields_ = [("tokens_before", C.c_uint64), ("docs_before", C.c_uint64), ("owned", C.c_uint32), ("holds_root", C.c_uint32), ("halo_before", C.c_uint32),
+                ("halo_after", C.c_uint32), ("halo_flags", C.c_uint32), ("last_type", C.c_uint32)]
+
+
+class GrammarEdgeFoldResult(C.Structure):
+    _fields_ = [("error", C.c_int), ("bad_table", C.c_uint32), ("n", C.c_uint64), ("ndocs", C.c_uint64)]
+
+
+class GrammarTally(C.Structure):
+    _fields_ = [("lead", C.c_uint64), ("last", C.c_uint64), ("first_key", C.c_uint64), ("errors", C.c_uint32), ("first_doc", C.c_uint32)]
+
+
 def load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
@@ -193,6 +221,12 @@ def load():
         "sjb200_tokens_sharded_finish": (C.c_int, [vp, C.POINTER(ShardedTokensResult)]),
         "sjb200_at_pointer_dev": (C.c_int, [vp, vp, vp, C.c_uint32, vp, sz, vp, C.c_uint32, vp, vp, C.c_int, vp, vp]),
         "sjb200_document_errors_dev": (C.c_int, [vp, vp, vp, C.c_uint32, vp, C.c_uint32, sz, vp, C.POINTER(DocumentErrorsResult), vp]),
+        "sjb200_document_errors_sharded": (C.c_int, [vp, vp, vp, C.c_uint32, C.c_int, vp, C.c_uint32, sz, vp, C.POINTER(ShardedDocumentErrorsResult), vp]),
+        "sjb200_document_errors_sharded_enqueue": (C.c_int, [vp, vp, vp, C.c_uint32, C.c_int, vp, C.c_uint32, sz, vp, vp]),
+        "sjb200_document_errors_sharded_finish": (C.c_int, [vp, C.POINTER(ShardedDocumentErrorsResult)]),
+        "sjb200_grammar_edge_fold": (C.c_int, [C.c_int, C.POINTER(GrammarEdge), C.POINTER(GrammarEdgeFoldResult), C.POINTER(GrammarRank)]),
+        "sjb200_grammar_result_fold": (C.c_int, [C.c_int, C.POINTER(GrammarEdge), C.POINTER(GrammarTally), C.POINTER(ShardedDocumentErrorsResult),
+                                                 C.POINTER(ShardedDocumentError)]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)

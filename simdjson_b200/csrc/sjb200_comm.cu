@@ -8,6 +8,7 @@
 
 #include "sjb200_bits.cuh"
 #include "sjb200_ctx.h"
+#include "sjb200_grammar.h"
 #include "sjb200_kernels.cuh"
 
 using namespace sjb200;
@@ -81,7 +82,7 @@ struct sjb200_comm {
   unsigned long long *peer[kMaxRanks] = {};        // peer[r] = rank r's window as seen from this device
   bool opened[kMaxRanks] = {};                     // mapped through cudaIpcOpenMemHandle (to be closed)
   bool connected = false;
-  unsigned long long *h_rec = nullptr;             // pinned [kMaxRanks][kDelimWords]: records ([r][0..1]), summaries or delimited blocks
+  unsigned long long *h_rec = nullptr;             // pinned [kMaxRanks][kGramWords]: records ([r][0..1]), summaries, delimited or grammar blocks
   uint32_t *h_tot = nullptr;                       // pinned [4]: a delimited pass's filter totals
   uint32_t *d_scratch = nullptr;                   // a delimited pass's filter scratch (delim_scratch_words)
   size_t scratch_words = 0;
@@ -90,6 +91,13 @@ struct sjb200_comm {
   TokenTotals *d_tok_tot = nullptr;
   uint8_t *d_tok_scratch[kXchgSteps] = {};
   size_t tok_scratch_bytes[kXchgSteps] = {};
+  // grammar passes, by the slot of their pass: the call's arguments, scratch (grow-only)
+  struct GramStep {
+    const uint8_t *type; const uint64_t *payload; uint32_t n; bool whole; const sjb200_doc_boundary *docs; uint32_t ndocs; size_t max_depth;
+    sjb200_sharded_document_error *out;
+  } gram[kXchgSteps];
+  uint32_t *d_gram_scratch[kXchgSteps] = {};
+  size_t gram_scratch_words[kXchgSteps] = {};
   cudaStream_t poll_stream = nullptr;
   cudaEvent_t done[kXchgSteps] = {};
   struct Step {
@@ -102,6 +110,7 @@ struct sjb200_comm {
 
 namespace {
 constexpr size_t kWindowWords = kXchgWindowWords;
+constexpr size_t kHostWords = size_t(kMaxRanks) * (kGramWords > kDelimWords ? kGramWords : kDelimWords);  // h_rec
 uint32_t window_slot(uint32_t seq, int round) { return (seq % uint32_t(kXchgSteps)) * 2u + uint32_t(round); }
 
 // Where this rank's launches of pass `seq` store their words.  Rounds 0 and 1 are records, in their window slot; the
@@ -118,13 +127,15 @@ Xchg comm_target(const sjb200_comm *m, uint32_t seq, int round) {
 // wait (host polling, bounded) until every rank's record of (seq, round) is in the local window; records -> comm->h_rec.
 // round 2: the summaries of a streaming pass (kSumWords words per rank, each tagged with seq).  round 3: words
 // [first, first + nwords) of every rank's delimited block (h_rec[r * kDelimWords + k], the whole blocks are copied).
+// round 4: the same of every rank's grammar block (h_rec[r * kGramWords + k]).
 int comm_collect(sjb200_comm *m, uint32_t seq, int round, int first = 0, int nwords = 0) {
   sjb200_ctx *c = m->ctx;
-  const bool sums = (round == 2), delim = (round == 3);
-  const unsigned long long *src = delim  ? m->window + xchg_delim_at(seq, 0)
+  const bool sums = (round == 2), gram = (round == 4), delim = (round == 3) || gram;
+  const unsigned long long *src = gram   ? m->window + xchg_gram_at(seq, 0)
+                                  : delim ? m->window + xchg_delim_at(seq, 0)
                                   : sums ? m->window + xchg_summary_at(seq, 0)
                                          : m->window + size_t(window_slot(seq, round)) * kMaxRanks * 2;
-  const size_t words = delim ? size_t(kDelimWords) : sums ? size_t(kSumWords) : 2;
+  const size_t words = gram ? size_t(kGramWords) : delim ? size_t(kDelimWords) : sums ? size_t(kSumWords) : 2;
   const auto t0 = std::chrono::steady_clock::now();
   for (;;) {
     if (!ok(c, cudaMemcpyAsync(m->h_rec, src, size_t(m->nranks) * words * 8, cudaMemcpyDeviceToHost, m->poll_stream), "D2H window") ||
@@ -134,7 +145,7 @@ int comm_collect(sjb200_comm *m, uint32_t seq, int round, int first = 0, int nwo
     bool all = true;
     for (int r = 0; r < m->nranks; r++) {
       if (delim) {
-        for (int k = first; k < first + nwords; k++) all = all && uint32_t(m->h_rec[size_t(r) * kDelimWords + k] >> 32) == seq;
+        for (int k = first; k < first + nwords; k++) all = all && uint32_t(m->h_rec[size_t(r) * words + k] >> 32) == seq;
         continue;
       }
       if (!sums) { all = all && xchg_complete(m->h_rec[2 * r], m->h_rec[2 * r + 1], seq); continue; }
@@ -163,10 +174,10 @@ extern "C" int sjb200_comm_create(sjb200_ctx *c, int rank, int nranks, sjb200_co
   bool good = dev_alloc(c, &m->window, kWindowWords, "cudaMalloc(window)") &&
               ok(c, cudaMemset(m->window, 0, kWindowWords * sizeof(unsigned long long)), "memset window") &&
               dev_alloc(c, &m->d_result, kXchgSteps, "cudaMalloc(results)") &&
-              ok(c, cudaMallocHost(&hp, kMaxRanks * kDelimWords * 8 + 16), "cudaMallocHost") &&
+              ok(c, cudaMallocHost(&hp, kHostWords * 8 + 16), "cudaMallocHost") &&
               ok(c, cudaStreamCreateWithFlags(&m->poll_stream, cudaStreamNonBlocking), "stream");
   m->h_rec = static_cast<unsigned long long *>(hp);
-  if (hp) m->h_tot = reinterpret_cast<uint32_t *>(m->h_rec + kMaxRanks * kDelimWords);
+  if (hp) m->h_tot = reinterpret_cast<uint32_t *>(m->h_rec + kHostWords);
   for (int i = 0; good && i < kXchgSteps; i++) good = ok(c, cudaEventCreateWithFlags(&m->done[i], cudaEventDisableTiming), "event");
   if (!good) { sjb200_comm_destroy(m); return SJB200_MEMALLOC; }
   m->peer[rank] = m->window;
@@ -183,6 +194,7 @@ extern "C" void sjb200_comm_destroy(sjb200_comm *m) {
     if (m->opened[r] && m->peer[r]) cudaIpcCloseMemHandle(m->peer[r]);
   cudaFree(m->window); cudaFree(m->d_result); cudaFree(m->d_scratch); cudaFree(m->d_tok_tot);
   for (uint8_t *p : m->d_tok_scratch) cudaFree(p);
+  for (uint32_t *p : m->d_gram_scratch) cudaFree(p);
   if (m->h_rec) cudaFreeHost(m->h_rec);
   if (m->poll_stream) cudaStreamDestroy(m->poll_stream);
   for (auto e : m->done) if (e) cudaEventDestroy(e);
@@ -698,4 +710,135 @@ extern "C" int sjb200_tokens_sharded(sjb200_comm *m, const uint8_t *d_shard, siz
   int rc = sjb200_tokens_sharded_enqueue(m, d_shard, len, state_in, d_idx, n, d_type, d_payload, d_strbuf, strbuf_capacity, stream);
   if (rc != SJB200_SUCCESS) return rc;
   return sjb200_tokens_sharded_finish(m, out);
+}
+
+// ---------------------------------------------------------------------------------------------- sharded stage-2 grammar
+// Enqueue one grammar pass: the table's check and start bitmap, then the edge words and the round-0 record into every
+// rank's window.  Passes A-C wait for finish, which knows the halo.  A rank that cannot run its pass (bad arguments,
+// device allocation) still publishes, flagged, so that every rank's finish fails alike instead of waiting for it.
+extern "C" int sjb200_document_errors_sharded_enqueue(sjb200_comm *m, const uint8_t *d_type, const uint64_t *d_payload, uint32_t n, int whole,
+                                                      const sjb200_doc_boundary *d_docs, uint32_t ndocs, size_t max_depth,
+                                                      sjb200_sharded_document_error *d_out, void *stream) {
+  if (!m || !m->connected) return SJB200_UNEXPECTED_ERROR;
+  sjb200_comm::Step *st = pass_begin(m, kGrammar, 0, 0, nullptr, 0, nullptr, nullptr, stream);
+  if (!st) return SJB200_CAPACITY;
+  static_assert(sizeof(sjb200_sharded_document_error) == sizeof(gram::sjb200_sharded_document_error_t), "layout");
+  sjb200_ctx *c = m->ctx;
+  DeviceGuard g(c->device);
+  const uint32_t i = m->head % uint32_t(kXchgSteps);
+  if (whole) ndocs = 0;
+  bool failed = (n && (!d_type || !d_payload)) || (ndocs && !d_docs) || (!d_out && (whole ? m->rank == 0 : ndocs > 0));
+  if (failed) c->last_error = "sharded grammar pass: bad arguments";
+  const uint32_t md = max_depth == 0 ? 1u : max_depth > gram::kMaxDepth ? gram::kMaxDepth : uint32_t(max_depth);  // (CAPACITY is decided in finish)
+  gram::GrammarArgs a{};
+  a.type = d_type; a.payload = d_payload; a.n = n;
+  a.docs = ndocs ? reinterpret_cast<const sjb200_doc_boundary_t *>(d_docs) : nullptr;
+  a.ndocs = ndocs; a.max_depth = md;
+  failed = failed || !grow(c, &m->d_gram_scratch[i], &m->gram_scratch_words[i], gram::shard_scratch_words(n, ndocs, md), "cudaMalloc(grammar scratch)");
+  m->gram[i] = sjb200_comm::GramStep{d_type, d_payload, n, whole != 0, d_docs, ndocs, max_depth, d_out};
+  int launched = 0;
+  const bool good = ok(c, gram::launch_shard_edges(a, whole != 0, max_depth > 0xFFFFFFFFull ? 0xFFFFFFFFu : uint32_t(max_depth), failed, m->d_gram_scratch[i],
+                                                    comm_target(m, st->seq, 0), xchg_gram_at(st->seq, uint32_t(m->rank)), st->stream, &launched),
+                       "grammar edges");
+  c->launches += unsigned(launched);
+  return pass_end(m, good);
+}
+
+// Complete the oldest pass in flight, a grammar pass: round 0 (kind), the edge round and its fold (errors every rank sees
+// alike, the halo, the bases), then pass A and the fold tree up with the record round, then the incoming stack, the
+// fold tree down, pass C and the result round, whose fold gives the last document's result and the counts.
+extern "C" int sjb200_document_errors_sharded_finish(sjb200_comm *m, sjb200_sharded_document_errors_result *out) {
+  if (!m || !out || m->tail == m->head) return SJB200_UNEXPECTED_ERROR;
+  sjb200_ctx *c = m->ctx;
+  DeviceGuard g(c->device);
+  memset(out, 0, sizeof(*out));
+  out->error = SJB200_UNEXPECTED_ERROR;
+  out->first_doc_in_error = out->first_error_index = UINT64_MAX;
+  const uint32_t slot = m->tail % uint32_t(kXchgSteps);
+  sjb200_comm::Step st;
+  int rc = pass_pop(m, kGrammar, &st);
+  if (rc != SJB200_SUCCESS) return rc;
+  const sjb200_comm::GramStep gs = m->gram[slot];
+  const int me = m->rank, R = m->nranks;
+  if ((rc = comm_collect(m, st.seq, 4, kGramEdgeAt, kGramEdgeWords)) != SJB200_SUCCESS) return rc;
+  sjb200_grammar_edge e[kMaxRanks];
+  for (int r = 0; r < R; r++) {
+    const unsigned long long *w = m->h_rec + size_t(r) * kGramWords + kGramEdgeAt;
+    e[r] = sjb200_grammar_edge{uint32_t(w[0]), uint32_t(w[1]), uint32_t(w[2]), uint32_t(w[3]), uint32_t(w[4]), uint32_t(w[5])};
+  }
+  sjb200_grammar_edge_fold_result res;
+  sjb200_grammar_rank ranks[kMaxRanks];
+  int err = sjb200_grammar_edge_fold(R, e, &res, ranks);
+  out->docs_before = ranks[me].docs_before;
+  out->tokens_before = ranks[me].tokens_before;
+  if (err != SJB200_SUCCESS) {
+    int failed = -1;
+    for (int r = 0; r < R && failed < 0; r++)
+      if (e[r].flags & kGramEdgeFailed) failed = r;
+    if (failed >= 0 && failed != me)
+      c->last_error = "sharded grammar pass " + std::to_string(st.seq) + ": rank " + std::to_string(failed) + " could not run its pass";
+    else if (failed < 0 && err == SJB200_UNEXPECTED_ERROR)
+      c->last_error = "sharded grammar pass " + std::to_string(st.seq) + ": the ranks disagree on whole or max_depth";
+    out->error = err;
+    return err;
+  }
+  out->ndocs = res.ndocs;
+  out->error = SJB200_SUCCESS;
+  if (!gs.whole && res.ndocs == 0) return SJB200_SUCCESS;  // no document on any rank: nothing to judge
+  cudaStream_t s = m->poll_stream;
+  gram::ShardPass p{};
+  p.a.type = gs.type; p.a.payload = gs.payload; p.a.n = gs.n;
+  p.a.docs = gs.ndocs ? reinterpret_cast<const sjb200_doc_boundary_t *>(gs.docs) : nullptr;
+  p.a.ndocs = gs.ndocs; p.a.max_depth = uint32_t(gs.max_depth);
+  p.whole = gs.whole;
+  p.owned = ranks[me].owned;
+  p.tokens_before = ranks[me].tokens_before;
+  p.out = reinterpret_cast<gram::sjb200_sharded_document_error_t *>(gs.out);
+  if (res.bad_table) {  // every result {UNEXPECTED_ERROR, none}
+    if (!ok(c, gram::launch_shard_fill_bad(p, s), "grammar results") || !ok(c, cudaStreamSynchronize(s), "sync")) return SJB200_UNEXPECTED_ERROR;
+    c->launches += p.owned ? 1 : 0;
+    c->last_error = "sharded grammar pass: a rank's document table is not strictly ascending or has an entry at or above its n";
+    out->ndocs_in_error = res.ndocs;
+    out->first_doc_in_error = res.ndocs ? 0 : UINT64_MAX;
+    out->first_error = res.ndocs ? SJB200_UNEXPECTED_ERROR : SJB200_SUCCESS;
+    out->error = SJB200_UNEXPECTED_ERROR;
+    return SJB200_UNEXPECTED_ERROR;
+  }
+  const gram::ShardHalo h{ranks[me].halo_before, ranks[me].halo_after, ranks[me].halo_flags, ranks[me].last_type};
+  const Xchg x = comm_target(m, st.seq, 2);
+  const size_t at = xchg_gram_at(st.seq, uint32_t(me));
+  uint32_t *scratch = m->d_gram_scratch[slot];
+  int launched = 0;
+  // record round
+  if (!ok(c, gram::launch_shard_records(p, h, ranks[me].holds_root != 0, scratch, c->sm_count, x, at, s, &launched), "grammar records"))
+    return SJB200_UNEXPECTED_ERROR;
+  c->launches += unsigned(launched);
+  if ((rc = comm_collect(m, st.seq, 4, kGramRecAt, 2 + int((p.a.max_depth + 31) / 32))) != SJB200_SUCCESS) return rc;
+  // result round
+  if (!ok(c, gram::launch_shard_check(p, h, scratch, m->window + xchg_gram_at(st.seq, 0), c->sm_count, x, at, s, &launched), "grammar check"))
+    return SJB200_UNEXPECTED_ERROR;
+  c->launches += unsigned(launched);
+  if ((rc = comm_collect(m, st.seq, 4, kGramResAt, kGramResWords)) != SJB200_SUCCESS) return rc;
+  sjb200_grammar_tally t[kMaxRanks];
+  for (int r = 0; r < R; r++) {
+    const unsigned long long *w = m->h_rec + size_t(r) * kGramWords + kGramResAt;
+    auto u64 = [&](int k) { return uint64_t(uint32_t(w[k])) | (uint64_t(uint32_t(w[k + 1])) << 32); };
+    t[r] = sjb200_grammar_tally{u64(0), u64(2), u64(6), uint32_t(w[4]), uint32_t(w[5])};
+  }
+  sjb200_sharded_document_error last[kMaxRanks];
+  err = sjb200_grammar_result_fold(R, e, t, out, last);
+  out->docs_before = ranks[me].docs_before;
+  out->tokens_before = ranks[me].tokens_before;
+  if (p.owned && !ok(c, gram::launch_shard_store(p.out + (p.owned - 1), last[me].error, last[me].index, s), "grammar result")) return SJB200_UNEXPECTED_ERROR;
+  c->launches += p.owned ? 1 : 0;
+  if (!ok(c, cudaStreamSynchronize(s), "sync")) return SJB200_UNEXPECTED_ERROR;
+  return err;
+}
+
+extern "C" int sjb200_document_errors_sharded(sjb200_comm *m, const uint8_t *d_type, const uint64_t *d_payload, uint32_t n, int whole,
+                                              const sjb200_doc_boundary *d_docs, uint32_t ndocs, size_t max_depth, sjb200_sharded_document_error *d_out,
+                                              sjb200_sharded_document_errors_result *out, void *stream) {
+  int rc = sjb200_document_errors_sharded_enqueue(m, d_type, d_payload, n, whole, d_docs, ndocs, max_depth, d_out, stream);
+  if (rc != SJB200_SUCCESS) return rc;
+  return sjb200_document_errors_sharded_finish(m, out);
 }

@@ -263,3 +263,114 @@ extern "C" size_t sjb200_shard_cut_line(const uint8_t *buf, size_t len, size_t n
     if (buf[cut - 1] == 0x0A) return cut;
   return sjb200_shard_cut(buf, len, nominal);
 }
+
+// ---- sharded grammar (sjb200_document_errors_sharded)
+namespace {
+constexpr uint32_t kEdgeFailed = 1, kEdgeBadTable = 2, kEdgeWhole = 4, kEdgeFirstStarts = 8, kEdgeLastStarts = 16;
+uint32_t type_byte(uint32_t types, int b) { return (types >> (8 * b)) & 0xFFu; }
+}  // namespace
+
+// The edge round: every rank's place in the stream and the halo of its structurals.  A rank's neighbours k - 2, k - 1
+// and k + 1 may lie on any other rank, past ranks with n = 0 or 1.
+extern "C" int sjb200_grammar_edge_fold(int nranks, const sjb200_grammar_edge *e, sjb200_grammar_edge_fold_result *res, sjb200_grammar_rank *ranks) {
+  if (!e || !res || !ranks || nranks < 1 || nranks > kMaxRanks) return SJB200_UNEXPECTED_ERROR;
+  memset(res, 0, sizeof(*res));
+  memset(ranks, 0, sizeof(*ranks) * size_t(nranks));
+  bool failed = false, capacity = false, differ = false;
+  const bool whole = (e[0].flags & kEdgeWhole) != 0;
+  for (int r = 0; r < nranks; r++) {
+    failed = failed || (e[r].flags & kEdgeFailed);
+    capacity = capacity || e[r].max_depth == 0 || e[r].max_depth > SJB200_DOCUMENT_MAX_DEPTH;
+    differ = differ || e[r].max_depth != e[0].max_depth || ((e[r].flags & kEdgeWhole) != 0) != whole;
+    if (!whole && (e[r].flags & kEdgeBadTable)) res->bad_table = 1;
+  }
+  res->error = failed ? SJB200_UNEXPECTED_ERROR : capacity ? SJB200_CAPACITY : differ ? SJB200_UNEXPECTED_ERROR : SJB200_SUCCESS;
+  uint64_t tokens = 0, docs = 0;
+  for (int r = 0; r < nranks; r++) {
+    sjb200_grammar_rank &k = ranks[r];
+    k.tokens_before = tokens;
+    k.docs_before = docs;
+    k.owned = whole ? (r == 0 ? 1u : 0u) : e[r].ndocs;
+    k.holds_root = tokens == 0 && e[r].n > 0;
+    tokens += e[r].n;
+    docs += k.owned;
+  }
+  res->n = tokens;
+  res->ndocs = docs;
+  // does rank q's structural j (0 or n - 1) start a document
+  auto starts = [&](int q, bool last) {
+    if (ranks[q].holds_root && (!last || e[q].n == 1)) return true;
+    return !whole && (e[q].flags & (last ? kEdgeLastStarts : kEdgeFirstStarts)) != 0;
+  };
+  uint32_t last_type = 0xFFu;
+  for (int r = 0; r < nranks; r++)
+    if (e[r].n) last_type = type_byte(e[r].types, 3);
+  for (int r = 0; r < nranks; r++) {
+    sjb200_grammar_rank &k = ranks[r];
+    uint32_t before[2] = {0xFFu, 0xFFu};  // [0] the structural just before, [1] the one before it
+    int got = 0, prev = -1;
+    for (int q = r - 1; q >= 0 && got < 2; q--) {
+      if (!e[q].n) continue;
+      if (prev < 0) prev = q;
+      before[got++] = type_byte(e[q].types, 3);
+      if (got < 2 && e[q].n >= 2) before[got++] = type_byte(e[q].types, 2);
+    }
+    int next = -1;
+    for (int q = r + 1; q < nranks && next < 0; q++)
+      if (e[q].n) next = q;
+    k.halo_before = before[1] | (before[0] << 8) | 0xFFFF0000u;
+    k.halo_after = next < 0 ? 0xFFu : type_byte(e[next].types, 0);
+    k.halo_flags = (prev >= 0 && starts(prev, true) ? 1u : 0u) | (next >= 0 && starts(next, false) ? 2u : 0u) | (k.holds_root ? 4u : 0u);
+    k.last_type = last_type;
+  }
+  return res->error;
+}
+
+// The result round: a document that spans ranks is owned by the rank it starts on, and its error is the first in rank
+// order over the ranks it spans -- its owner's own, then the leading segments of the ranks up to the next start.
+extern "C" int sjb200_grammar_result_fold(int nranks, const sjb200_grammar_edge *e, const sjb200_grammar_tally *t,
+                                          sjb200_sharded_document_errors_result *out, sjb200_sharded_document_error *last) {
+  if (!e || !t || !out || !last || nranks < 1 || nranks > kMaxRanks) return SJB200_UNEXPECTED_ERROR;
+  sjb200_grammar_edge_fold_result res;
+  sjb200_grammar_rank ranks[kMaxRanks];
+  sjb200_grammar_edge_fold(nranks, e, &res, ranks);
+  const bool whole = (e[0].flags & kEdgeWhole) != 0;
+  const uint64_t none = ~0ull;
+  uint64_t key[kMaxRanks];
+  int owner = -1;
+  for (int r = 0; r < nranks; r++) {
+    if (owner >= 0 && t[r].lead < key[owner]) key[owner] = t[r].lead;
+    if (ranks[r].owned) {
+      owner = r;
+      key[r] = t[r].last;
+    }
+  }
+  if (whole && res.n == 0) key[0] = uint64_t(SJB200_EMPTY);  // {EMPTY, 0}
+  out->error = SJB200_SUCCESS;
+  out->first_error = SJB200_SUCCESS;
+  out->ndocs = res.ndocs;
+  out->ndocs_in_error = 0;
+  out->first_doc_in_error = none;
+  out->first_error_index = none;
+  for (int r = 0; r < nranks; r++) {
+    if (!ranks[r].owned) continue;
+    uint64_t next = res.n;  // one past the last document's value when it is good: the next document's start
+    for (int q = r + 1; q < nranks && !whole; q++)
+      if (ranks[q].owned) { next = ranks[q].tokens_before + e[q].first_start; break; }
+    last[r].error = key[r] == none ? 0 : int32_t(key[r] & 0xFFu);
+    last[r].reserved = 0;
+    last[r].index = key[r] == none ? next : key[r] >> 8;
+    out->ndocs_in_error += t[r].errors + (key[r] != none ? 1u : 0u);
+    if (out->first_doc_in_error != none) continue;
+    if (t[r].first_doc != 0xFFFFFFFFu) {
+      out->first_doc_in_error = ranks[r].docs_before + t[r].first_doc;
+      out->first_error = int32_t(t[r].first_key & 0xFFu);
+      out->first_error_index = t[r].first_key >> 8;
+    } else if (key[r] != none) {
+      out->first_doc_in_error = ranks[r].docs_before + ranks[r].owned - 1;
+      out->first_error = last[r].error;
+      out->first_error_index = last[r].index;
+    }
+  }
+  return out->error;
+}

@@ -19,6 +19,7 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include "sjb200_params.h"
 #include "sjb200_simt.cuh"
 
 namespace sjb200 {
@@ -54,8 +55,40 @@ SJ_DEV bool is_scalar(uint32_t t) { return t == '"' || t == 'l' || t == 'u' || t
 SJ_DEV uint32_t closer_of(uint32_t t) { return t == '{' ? '}' : ']'; }
 SJ_DEV bool start_at(const uint32_t *starts, uint32_t k) { return (sj_ldg_u32(starts + (k >> 5)) >> (k & 31u)) & 1u; }
 
-// A tile's structurals in shared memory: ty[i + 2] = type of structural tile0 + i (halo: two before, one after; 0xFF past
-// the ends), dep[i] = its depth D before it, lane_min[l] = the lowest depth among lane l's structurals.
+// What lies around the structurals [0, n) of a Grammar.  NoHalo: nothing -- the whole stream (sjb200_document_errors_dev);
+// the tile routines then do exactly what they did before halos existed.  ShardHalo: one rank's shard of a sharded pass
+// (sjb200_document_errors_sharded): the neighbours of its first and last structurals, which may lie on any other rank.
+struct NoHalo {
+  SJ_DEV uint8_t type_outside(const Grammar &, uint32_t) const { return 0xFF; }
+  SJ_DEV bool pair_across(const Grammar &, uint32_t, bool) const { return false; }
+  SJ_DEV bool start_before(const Grammar &g, uint32_t k) const { return start_at(g.starts, k - 1); }
+  SJ_DEV bool ends_at(const Grammar &, uint32_t) const { return true; }
+  SJ_DEV uint32_t last_type(const Grammar &g) const { return g.whole ? sj_ldg_u8(g.type + g.n - 1) : 0u; }
+  SJ_DEV bool root_at(uint32_t k) const { return k == 0; }
+};
+
+struct ShardHalo {
+  static constexpr uint32_t kPrevStart = 1, kNextStart = 2, kRoot = 4;
+  uint32_t before;  // types of the two structurals before structural 0: byte 0 the one two before, byte 1 the one just before (0xFF: none)
+  uint32_t after;   // type of the structural after n - 1 (0xFF: none)
+  uint32_t flags;   // kPrevStart: the structural before 0 starts a document; kNextStart: the one after n - 1 does; kRoot: 0 is the stream's first
+  uint32_t last;    // whole mode: type of the stream's last structural
+  // type of tile slot p = k + 2 outside [0, n): the halo before (p < 2) or after (p == n + 2)
+  SJ_DEV uint8_t type_outside(const Grammar &g, uint32_t p) const {
+    if (p < 2) return uint8_t(before >> (8u * p));
+    return uint64_t(p) == uint64_t(g.n) + 2 ? uint8_t(after) : uint8_t(0xFF);
+  }
+  // an opener at n - 1 and the closer after the cut are an empty pair (closes: that closer matches the opener)
+  SJ_DEV bool pair_across(const Grammar &g, uint32_t k, bool closes) const { return k + 1 == g.n && closes && !(flags & kNextStart); }
+  SJ_DEV bool start_before(const Grammar &g, uint32_t k) const { return k ? start_at(g.starts, k - 1) : (flags & kPrevStart) != 0; }
+  // false when structural n - 1 looks like a document's end only because the shard ends there
+  SJ_DEV bool ends_at(const Grammar &g, uint32_t k) const { return k + 1 != g.n || after == 0xFFu || (flags & kNextStart) != 0; }
+  SJ_DEV uint32_t last_type(const Grammar &) const { return last; }
+  SJ_DEV bool root_at(uint32_t k) const { return k == 0 && (flags & kRoot) != 0; }
+};
+
+// A tile's structurals in shared memory: ty[i + 2] = type of structural tile0 + i (halo: two before, one after; past the
+// ends the halo's types, 0xFF without one), dep[i] = its depth D before it, lane_min[l] = the lowest depth among lane l's structurals.
 template <int ITEMS>
 struct TileSmem {
   static constexpr uint32_t kTile = 32u * ITEMS;
@@ -68,20 +101,20 @@ struct TileSmem {
 
 // The tile's types, and per structural its depth change: +1 a non-empty opener, -1 a closer that does not end an empty
 // pair.  An empty pair is an opener followed, in the same document, by its own closer.
-template <int ITEMS>
-SJ_DEV void load_tile(const Grammar &g, TileSmem<ITEMS> &sm, unsigned lane, uint32_t tile0) {
+template <int ITEMS, class H = NoHalo>
+SJ_DEV void load_tile(const Grammar &g, TileSmem<ITEMS> &sm, unsigned lane, uint32_t tile0, const H &h = H()) {
   for (uint32_t i = lane; i < TileSmem<ITEMS>::kTile + 3; i += 32) {
     const uint64_t k = uint64_t(tile0) + i - 2;  // wraps below 0: past the end too
-    sm.ty[i] = uint64_t(tile0) + i >= 2 && k < g.n ? uint8_t(sj_ldg_u8(g.type + k)) : uint8_t(0xFF);
+    sm.ty[i] = uint64_t(tile0) + i >= 2 && k < g.n ? uint8_t(sj_ldg_u8(g.type + k)) : h.type_outside(g, tile0 + i);
   }
   sj_syncwarp();
 }
 
-template <int ITEMS>
-SJ_DEV int delta_at(const Grammar &g, const TileSmem<ITEMS> &sm, uint32_t tile0, uint32_t i) {
+template <int ITEMS, class H = NoHalo>
+SJ_DEV int delta_at(const Grammar &g, const TileSmem<ITEMS> &sm, uint32_t tile0, uint32_t i, const H &h = H()) {
   const uint32_t t = sm.ty[i + 2], k = tile0 + i;
   if (is_open(t)) {
-    const bool empty = k + 1 < g.n && sm.ty[i + 3] == closer_of(t) && !start_at(g.starts, k + 1);
+    const bool empty = (k + 1 < g.n && sm.ty[i + 3] == closer_of(t) && !start_at(g.starts, k + 1)) || h.pair_across(g, k, sm.ty[i + 3] == closer_of(t));
     return empty ? 0 : 1;
   }
   if (is_close(t)) {
@@ -94,8 +127,9 @@ SJ_DEV int delta_at(const Grammar &g, const TileSmem<ITEMS> &sm, uint32_t tile0,
 // Segmented depths of the tile: dep[i] = depth before structural tile0 + i, counted from the tile start for the
 // structurals before the tile's first document start, from that start (0) after it.  Returns the tile's first document
 // start (kNone: none) in *first_reset and its last in *last_reset.
-template <int ITEMS>
-SJ_DEV void tile_depths(const Grammar &g, TileSmem<ITEMS> &sm, unsigned lane, uint32_t tile0, uint32_t *first_reset, uint32_t *last_reset) {
+template <int ITEMS, class H = NoHalo>
+SJ_DEV void tile_depths(const Grammar &g, TileSmem<ITEMS> &sm, unsigned lane, uint32_t tile0, uint32_t *first_reset, uint32_t *last_reset,
+                        const H &h = H()) {
   const uint32_t i0 = lane * ITEMS;
   int d = 0;
   bool reset = false;
@@ -110,7 +144,7 @@ SJ_DEV void tile_depths(const Grammar &g, TileSmem<ITEMS> &sm, unsigned lane, ui
       lr = k;
     }
     sm.dep[i] = d;
-    d += delta_at(g, sm, tile0, i);
+    d += delta_at(g, sm, tile0, i, h);
   }
   // segmented exclusive scan over lanes of (reset, sum)
   uint32_t f = reset ? 1u : 0u;
@@ -137,10 +171,10 @@ SJ_DEV void tile_depths(const Grammar &g, TileSmem<ITEMS> &sm, unsigned lane, ui
 }
 
 // ---- pass A: the tile's stack record (of its last document segment)
-template <int ITEMS>
-SJ_DEV void tile_record(const Grammar &g, TileSmem<ITEMS> &sm, unsigned lane, uint32_t tile0, uint32_t *out) {
+template <int ITEMS, class H = NoHalo>
+SJ_DEV void tile_record(const Grammar &g, TileSmem<ITEMS> &sm, unsigned lane, uint32_t tile0, uint32_t *out, const H &h = H()) {
   uint32_t fr, lr;
-  tile_depths<ITEMS>(g, sm, lane, tile0, &fr, &lr);
+  tile_depths<ITEMS>(g, sm, lane, tile0, &fr, &lr, h);
   const uint32_t seg0 = lr == kNone ? tile0 : lr;  // the last segment
   const uint32_t i0 = lane * ITEMS;
   const uint32_t cap = g.words * 32u;
@@ -151,7 +185,7 @@ SJ_DEV void tile_record(const Grammar &g, TileSmem<ITEMS> &sm, unsigned lane, ui
     const uint32_t i = i0 + j, k = tile0 + i;
     if (k >= g.n) break;
     if (k < seg0) continue;
-    const int a = sm.dep[i] + delta_at(g, sm, tile0, i);
+    const int a = sm.dep[i] + delta_at(g, sm, tile0, i, h);
     lmin = a < lmin ? a : lmin;
     last_after = a;
   }
@@ -175,7 +209,7 @@ SJ_DEV void tile_record(const Grammar &g, TileSmem<ITEMS> &sm, unsigned lane, ui
   for (int j = ITEMS - 1; j >= 0; j--) {
     const uint32_t i = i0 + j, k = tile0 + i;
     if (k >= g.n || k < seg0) continue;
-    const int dl = delta_at(g, sm, tile0, i);
+    const int dl = delta_at(g, sm, tile0, i, h);
     const int a = sm.dep[i] + dl;
     if (dl == 1 && run >= a) {
       const uint32_t slot = uint32_t(a - m - 1);
@@ -280,10 +314,10 @@ SJ_DEV uint32_t value_error(const Grammar &g, uint32_t k, uint32_t t, bool empty
 
 // The first error of each document of the tile, as each lane sees it: report(pos, code, index) once per lane and document
 // segment, pos a structural of the document (index is one past it for a document that ends too early).
-template <int ITEMS, class F>
-SJ_DEV void tile_check(const Grammar &g, TileSmem<ITEMS> &sm, unsigned lane, uint32_t tile0, uint32_t tile, F &&report) {
+template <int ITEMS, class F, class H = NoHalo>
+SJ_DEV void tile_check(const Grammar &g, TileSmem<ITEMS> &sm, unsigned lane, uint32_t tile0, uint32_t tile, F &&report, const H &h = H()) {
   uint32_t fr, lr;
-  tile_depths<ITEMS>(g, sm, lane, tile0, &fr, &lr);
+  tile_depths<ITEMS>(g, sm, lane, tile0, &fr, &lr, h);
   const uint32_t *pre = g.prefix + size_t(tile) * (2 + g.words);
   const uint32_t d_in = pre[1];
   const uint32_t i0 = lane * ITEMS;
@@ -304,7 +338,7 @@ SJ_DEV void tile_check(const Grammar &g, TileSmem<ITEMS> &sm, unsigned lane, uin
   int before_min = int(sj_shfl_up(uint32_t(below), 1));
   if (lane == 0) before_min = 0x7FFFFFFF;
   sj_syncwarp();
-  const uint32_t last_type = g.whole ? sj_ldg_u8(g.type + g.n - 1) : 0u;
+  const uint32_t last_type = h.last_type(g);
   // the lane's own open containers (bit: '['), and one cached answer from below the lane
   uint32_t lbits = 0, lcnt = 0;
   int ext_level = -1;
@@ -353,7 +387,7 @@ SJ_DEV void tile_check(const Grammar &g, TileSmem<ITEMS> &sm, unsigned lane, uin
     }
     const uint32_t t = sm.ty[i + 2];
     const int D = sm.dep[i];
-    const int dl = delta_at(g, sm, tile0, i);
+    const int dl = delta_at(g, sm, tile0, i, h);
     if (seg_err == kNone) {
       // what the walk expects at k
       uint32_t exp;
@@ -369,7 +403,7 @@ SJ_DEV void tile_check(const Grammar &g, TileSmem<ITEMS> &sm, unsigned lane, uin
       } else if (p1 == ',') {
         exp = container(D) == '{' ? kExpKey : kExpValue;
       } else if (p1 == '"') {
-        const bool prev_start = start_at(g.starts, k - 1);
+        const bool prev_start = h.start_before(g, k);
         const uint32_t p2 = prev_start ? 0xFFu : sm.ty[i];
         exp = (!prev_start && (p2 == '{' || (p2 == ',' && container(D) == '{'))) ? kExpColon : kExpAfter;
       } else {
@@ -378,7 +412,7 @@ SJ_DEV void tile_check(const Grammar &g, TileSmem<ITEMS> &sm, unsigned lane, uin
       uint32_t code = 0;
       const bool empty = is_open(t) && dl == 0;
       if (exp == kExpRoot) {
-        if (g.whole && k == 0 && ((t == '{' && last_type != '}') || (t == '[' && last_type != ']'))) code = kTapeError;
+        if (g.whole && h.root_at(k) && ((t == '{' && last_type != '}') || (t == '[' && last_type != ']'))) code = kTapeError;
         else code = value_error(g, k, t, empty, D, true);
       } else if (exp == kExpValue) {
         code = value_error(g, k, t, empty, D, false);
@@ -406,7 +440,7 @@ SJ_DEV void tile_check(const Grammar &g, TileSmem<ITEMS> &sm, unsigned lane, uin
       lcnt--;
     }
     // the end of k's document: the walk must have finished its root value exactly here
-    const bool last = k + 1 == g.n || start_at(g.starts, k + 1);
+    const bool last = (k + 1 == g.n || start_at(g.starts, k + 1)) && h.ends_at(g, k);
     if (last && seg_err == kNone) {
       const bool done = D + dl == 0 && (is_scalar(t) || is_close(t));
       if (!done) {
@@ -418,6 +452,72 @@ SJ_DEV void tile_check(const Grammar &g, TileSmem<ITEMS> &sm, unsigned lane, uin
   }
   flush();
   sj_syncwarp();
+}
+
+// ---- one rank of a sharded pass (sjb200_document_errors_sharded): the pieces its kernels (sjb200_grammar.cu) and the
+// host emulation (tests/grammar_shards_emul.cpp) share.
+
+// the edge words of the rank (sjb200_params.h): n, ndocs, kGramEdge* flags, max_depth, the types of structurals 0, 1,
+// n - 2, n - 1 (0xFF: none), the table's first entry.  first / last: the table's first and last entries (ndocs > 0).
+SJ_DEV void shard_edge_words(const uint8_t *type, uint32_t n, bool whole, uint32_t ndocs, uint32_t first, uint32_t last, bool bad, bool failed,
+                             uint32_t max_depth_word, uint32_t *w) {
+  w[0] = n; w[1] = whole ? 0u : ndocs; w[2] = 0; w[3] = max_depth_word; w[4] = 0xFFFFFFFFu; w[5] = 0;
+  if (failed) {
+    w[2] = kGramEdgeFailed;
+    return;
+  }
+  const bool table = !whole && ndocs;
+  w[2] = (whole ? kGramEdgeWhole : 0u) | (bad ? kGramEdgeBadTable : 0u) | (table && first == 0 ? kGramEdgeFirstStarts : 0u) |
+         (table && n && last == n - 1 ? kGramEdgeLastStarts : 0u);
+  if (n) {
+    const uint32_t t0 = sj_ldg_u8(type), tl = sj_ldg_u8(type + n - 1);
+    const uint32_t t1 = n >= 2 ? sj_ldg_u8(type + 1) : 0xFFu, tm = n >= 2 ? sj_ldg_u8(type + n - 2) : 0xFFu;
+    w[4] = t0 | (t1 << 8) | (tm << 16) | (tl << 24);
+  }
+  w[5] = table ? first : 0u;
+}
+
+// The stack entering rank `rank`: the records of ranks 0 .. rank - 1 folded in order into dst (2 + words words).  rec(r,
+// k) is word k of rank r's record; acc and child are the warp's shared scratch.
+template <class W>
+SJ_DEV void shard_incoming(unsigned lane, uint32_t *acc, uint32_t *child, W &&rec, uint32_t rank, uint32_t words, uint32_t *dst) {
+  if (lane < 2) acc[lane] = 0;
+  sj_syncwarp();
+  for (uint32_t r = 0; r < rank; r++) {
+    for (uint32_t k = lane; k < 2 + words; k += 32) child[k] = rec(r, k);
+    sj_syncwarp();
+    compose(lane, acc, child, words);
+  }
+  copy_record(lane, dst, acc);
+}
+
+// the slot of first[] that an error of document d (kNone: before the rank's first document start) goes to: the document,
+// or the leading segment's slot `owned`.  Whole mode: slot 0 is rank 0's document, or the leading segment elsewhere.
+SJ_DEV uint32_t shard_slot(bool whole, uint32_t d, uint32_t owned) { return whole ? 0u : (d == kNone ? owned : d); }
+
+// the result of a document that starts on the rank and ends on it: its first error (key = index << 8 | code, local), or
+// SUCCESS one past its value (next: the local start of the next document)
+SJ_DEV void shard_doc_result(unsigned long long key, uint64_t tokens_before, uint32_t next, int32_t *error, uint64_t *index) {
+  if (key != ~0ull) {
+    *error = int32_t(key & 0xFFu);
+    *index = tokens_before + (key >> 8);
+  } else {
+    *error = 0;
+    *index = tokens_before + next;
+  }
+}
+
+SJ_DEV unsigned long long shard_global_key(unsigned long long key, uint64_t tokens_before) {
+  return key == ~0ull ? key : key + (static_cast<unsigned long long>(tokens_before) << 8);
+}
+
+// the result words of the rank (sjb200_params.h): its leading segment's first error, its last document's (global keys),
+// its other documents in error and the first of them (first_doc, kNone: none) with its key
+SJ_DEV void shard_result_words(const unsigned long long *first, uint32_t owned, uint64_t tokens_before, uint32_t errors, uint32_t first_doc, uint32_t *w) {
+  const unsigned long long lead = shard_global_key(first[owned], tokens_before), last = owned ? shard_global_key(first[owned - 1], tokens_before) : ~0ull;
+  const unsigned long long fk = first_doc != kNone ? shard_global_key(first[first_doc], tokens_before) : ~0ull;
+  w[0] = uint32_t(lead); w[1] = uint32_t(lead >> 32); w[2] = uint32_t(last); w[3] = uint32_t(last >> 32);
+  w[4] = errors; w[5] = first_doc; w[6] = uint32_t(fk); w[7] = uint32_t(fk >> 32);
 }
 
 }  // namespace gram

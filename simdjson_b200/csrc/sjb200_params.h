@@ -20,8 +20,8 @@ constexpr int kXchgSteps = 64;                        // sharded passes whose ex
 
 // ---- scan kinds (kStream: a stage-1 pass of the sharded streaming modes; kDelim: one of the sharded RS / comma-delimited
 // modes.  Both scan like kIndex, only their records differ.  kTokens: a sharded stage-2-lite pass, whose record comes
-// from tile_scan_kernel, sjb200_tape.cu)
-enum : int { kIndex = 0, kMinify = 1, kUtf8 = 2, kStream = 3, kDelim = 4, kTokens = 5 };
+// from tile_scan_kernel, sjb200_tape.cu.  kGrammar: a sharded stage-2 grammar pass, sjb200_grammar.cu)
+enum : int { kIndex = 0, kMinify = 1, kUtf8 = 2, kStream = 3, kDelim = 4, kTokens = 5, kGrammar = 6 };
 // a kTokens record's flags: kFlagInternal (the rank could not run its pass), or this rank's string bytes exceed its
 // string buffer (it wrote no records)
 constexpr uint32_t kTokShortFlag = 8u;
@@ -109,8 +109,9 @@ struct ScanParams {
 #endif
 // one shard record as two independently tagged 64-bit words (8-byte stores are single transactions):
 //   w0 = seq[30:0] << 33 | count[32:0]        w1 = seq << 32 | kind << 24 | flags << 16 | ttable << 8 | state_out
-// kind (3 bits, 24-26) is the scan kind of the pass (kIndex 0, kMinify 1, kUtf8 2, kStream 3, kDelim 4, kTokens 5); count
-// is structurals (kIndex, kStream, kDelim), kept bytes (kMinify), 0 (kUtf8) or string bytes (kTokens, whose state_out
+// kind (3 bits, 24-26) is the scan kind of the pass (kIndex 0, kMinify 1, kUtf8 2, kStream 3, kDelim 4, kTokens 5,
+// kGrammar 6); count is structurals (kIndex, kStream, kDelim, kGrammar: the rank's tokens), kept bytes (kMinify), 0 (kUtf8)
+// or string bytes (kTokens, whose state_out
 // field carries the state the caller says the shard starts in).  Bit 26 was zero before kDelim existed, so the records of
 // the other kinds are unchanged.
 SJ_PARAMS_HD inline unsigned long long xchg_word0(uint32_t seq, uint64_t count) {
@@ -128,7 +129,8 @@ SJ_PARAMS_HD inline uint64_t xchg_count(unsigned long long w0) { return w0 & 0x1
 
 // The window: the records of the two rounds, [kXchgSteps][2][kMaxRanks][2] words, then the summary area of the streaming
 // passes' extra round, [kXchgSteps][kMaxRanks][kSumWords] words, then the area of the delimited passes' three extra
-// rounds, [kXchgSteps][kMaxRanks][kDelimWords] words (layout below).  A summary is kSumWords words seq << 32 | payload:
+// rounds, [kXchgSteps][kMaxRanks][kDelimWords] words, then that of the grammar passes' three rounds,
+// [kXchgSteps][kMaxRanks][kGramWords] words (layouts below).  A summary is kSumWords words seq << 32 | payload:
 //   0 shard length (after the trim)   1 byte of structural 0         2 byte of the last structural (kept or not)
 //   3 local index of the last internal document start   4 its byte  5 / 6 object / array bracket net (int32) from that
 //   start on, or over every kept structural when there is none
@@ -152,9 +154,24 @@ SJ_PARAMS_HD inline size_t xchg_summary_at(uint32_t seq, uint32_t rank) {
 //   tail round    24..26 the words n, n+1, n+2 of the whole call this rank holds (0 for the others)
 constexpr int kDelimWords = 32;
 enum : int { kDelimCarryAt = 0, kDelimCarryWords = 3, kDelimTotalsAt = 4, kDelimWalkAt = 8, kDelimWalkBelowAt = 16, kDelimTailAt = 24 };
-constexpr size_t kXchgWindowWords = kXchgRecordWords + kXchgSummaryWords + size_t(kXchgSteps) * kMaxRanks * kDelimWords;
+constexpr size_t kXchgDelimWords = size_t(kXchgSteps) * kMaxRanks * kDelimWords;
 SJ_PARAMS_HD inline size_t xchg_delim_at(uint32_t seq, uint32_t rank) {
   return kXchgRecordWords + kXchgSummaryWords + (size_t(seq % uint32_t(kXchgSteps)) * kMaxRanks + rank) * kDelimWords;
+}
+// A grammar pass's block of one rank (sjb200_document_errors_sharded), kGramWords words, each seq << 32 | payload:
+//   edge round    0 n   1 ndocs   2 kGramEdge* bits   3 max_depth (saturated to 32 bits)   4 types of structurals 0, 1,
+//                 n - 2, n - 1 (a byte each, 0xFF: none)   5 the table's first entry
+//   record round  8 .. 8 + 2 + ceil(max_depth / 32): the stack record of the whole shard (the top of its fold tree)
+//   result round  138 / 139 low / high half of the first error of the shard's leading continuation segment (global
+//                 index << 8 | code, all ones: none)   140 / 141 the same of its last document   142 its other documents
+//                 in error   143 the first of them (0xFFFFFFFF: none)   144 / 145 that one's error as 138 / 139
+constexpr int kGramWords = 146;
+enum : int { kGramEdgeAt = 0, kGramEdgeWords = 6, kGramRecAt = 8, kGramResAt = 138, kGramResWords = 8 };
+enum : uint32_t { kGramEdgeFailed = 1, kGramEdgeBadTable = 2, kGramEdgeWhole = 4, kGramEdgeFirstStarts = 8, kGramEdgeLastStarts = 16 };
+constexpr size_t kXchgGramWords = size_t(kXchgSteps) * kMaxRanks * kGramWords;
+constexpr size_t kXchgWindowWords = kXchgRecordWords + kXchgSummaryWords + kXchgDelimWords + kXchgGramWords;
+SJ_PARAMS_HD inline size_t xchg_gram_at(uint32_t seq, uint32_t rank) {
+  return kXchgRecordWords + kXchgSummaryWords + kXchgDelimWords + (size_t(seq % uint32_t(kXchgSteps)) * kMaxRanks + rank) * kGramWords;
 }
 
 }  // namespace sjb200

@@ -100,6 +100,7 @@ class Comm:
         self._capi = capi
         self.parser, self.rank, self.world = parser, rank, world
         self._tokens_out = collections.deque()  # the outputs of the tokens passes in flight, oldest first
+        self._grammar_out = collections.deque()  # ... and of the grammar passes
         self._h = C.c_void_p()
         rc = _lib().sjb200_comm_create(parser._ctx, rank, world, C.byref(self._h))
         if rc != 0:
@@ -258,6 +259,55 @@ class Comm:
         if rc != 0:
             return rc, None, None, None, None
         return self.tokens_finish()
+
+    # stage-2 grammar over this shard's tokens; its passes share the window with the other kinds
+    def document_errors_enqueue(self, d_type, d_payload, n, whole, table=None, max_depth=None, stream=None):
+        """(d_type, d_payload, n): this rank's output of a sharded tokens pass.  whole = True: the ranks hold one document;
+        else table is this rank's document table (a [ndocs, 2] array from document_table, or a device tensor of
+        sjb200_doc_boundary; None or empty: no document starts here).  Allocates d_out (one 16-byte result per document
+        that starts here) and keeps it until document_errors_finish returns it."""
+        import torch
+
+        from .implementation import _stream_ptr
+        n = int(n)
+        dev = d_type.device
+        max_depth = self.parser.max_depth if max_depth is None else int(max_depth)
+        d_docs, ndocs = None, 0
+        if not whole and table is not None and len(table):
+            if isinstance(table, torch.Tensor) and table.is_cuda:
+                d_docs, ndocs = table, table.numel() * table.element_size() // 8
+            else:
+                arr = np.ascontiguousarray(np.asarray(table, dtype=np.int64).reshape(-1, 2).astype(np.uint32)).view(np.int32).reshape(-1)
+                d_docs, ndocs = torch.from_numpy(arr.copy()).to(dev), len(arr) // 2
+        nout = 1 if whole else ndocs
+        d_out = torch.empty(max(nout, 1) * 2, dtype=torch.int64, device=dev)
+        rc = _lib().sjb200_document_errors_sharded_enqueue(self._h, d_type.data_ptr() if n else None, d_payload.data_ptr() if n else None, n, int(bool(whole)),
+                                                           d_docs.data_ptr() if ndocs else None, ndocs, max_depth, d_out.data_ptr(), _stream_ptr(stream))
+        if rc == 0:
+            self._grammar_out.append((d_out, d_docs, nout if (not whole or self.rank == 0) else 0))
+        return rc
+
+    def document_errors_finish(self):
+        """(error_code, ShardedDocumentErrorsResult, errors int32[k], indexes uint64[k]) of the oldest pass in flight: the
+        results of the k documents that start on this rank (whole mode: rank 0's one), global structural indexes"""
+        res = self._capi.ShardedDocumentErrorsResult()
+        rc = _lib().sjb200_document_errors_sharded_finish(self._h, C.byref(res))
+        if rc == self._capi.UNEXPECTED_ERROR and "oldest pass in flight is of another kind" in self.parser.last_cuda_error():
+            return rc, res, None, None
+        d_out, _, k = self._grammar_out.popleft() if self._grammar_out else (None, None, 0)
+        # d_out holds results on success, and after a bad table (every result UNEXPECTED_ERROR); else nothing was written
+        written = rc == 0 or (rc == self._capi.UNEXPECTED_ERROR and res.ndocs > 0 and res.ndocs_in_error == res.ndocs
+                              and res.first_error == self._capi.UNEXPECTED_ERROR)
+        if d_out is None or not written or res.ndocs == 0:
+            return rc, res, np.zeros(0, dtype=np.int32), np.zeros(0, dtype=np.uint64)
+        out = d_out[: 2 * k].cpu().numpy().view(np.uint64).reshape(-1, 2)
+        return rc, res, (out[:, 0] & 0xFFFFFFFF).astype(np.uint32).view(np.int32), out[:, 1].copy()
+
+    def document_errors(self, d_type, d_payload, n, whole, table=None, max_depth=None, stream=None):
+        rc = self.document_errors_enqueue(d_type, d_payload, n, whole, table, max_depth, stream)
+        if rc != 0:
+            return rc, None, None, None
+        return self.document_errors_finish()
 
     def document_table(self, d_shard, d_idx, result, stream=None):
         """the document starts among this shard's kept structurals (result: a ShardedStreamResult, or the `stream` field of
