@@ -493,6 +493,53 @@ SJB200_API int sjb200_document_errors_sharded(sjb200_comm *comm, const uint8_t *
                                               const sjb200_doc_boundary *d_docs, uint32_t ndocs, size_t max_depth,
                                               sjb200_sharded_document_error *d_out, sjb200_sharded_document_errors_result *out, void *stream);
 
+/* JSON Pointer lookup (sjb200_at_pointer_dev) sharded the same way, on the same comm and window: every rank walks the
+ * documents that start on it, and a walk that reaches the end of a rank inside its document is handed, as a small
+ * record, to the next rank that holds structurals, which resumes it.  A pointer pass has its own kind.  (d_type,
+ * d_payload, n, d_strbuf, string_bytes) is this rank's output of sjb200_tokens_sharded; string payloads and d_strbuf stay
+ * rank-local.  n may be 0.
+ *   whole = 1: the ranks together hold ONE document; d_docs / ndocs are ignored.
+ *   whole = 0: d_docs / ndocs is this rank's table from sjb200_document_table_shard_dev (ndocs may be 0: a rank inside
+ *              one long document).
+ * Every rank passes the same whole and the same pointers.  The contract: gather the inputs -- the concatenations of the
+ * ranks' types, payloads ('"' payloads + string_base), string buffers and tables (index + tokens_before) -- and run
+ * sjb200_at_pointer_dev on them (no table in whole mode).  Rank r's d_out[p * ndocs + j] (device memory) is that call's
+ * result for pointer p and document docs_before + j, the j-th document that STARTS on rank r; in whole mode rank 0
+ * writes the npointers results.  Indexes are global and 64-bit (0xFFFFFFFF there is UINT64_MAX here).  For a document
+ * that spans ranks the first token in error is the first over all of its pieces.  Two exceptions: a bad table on any
+ * rank makes every result {UNEXPECTED_ERROR, UINT64_MAX} (where a document on one rank ends depends on the others'
+ * tables); whole = 0 with no document on any rank writes nothing, reports 0 documents and returns SUCCESS.
+ * finish returns, on every rank alike: CAPACITY (nothing written) when a rank has more than
+ * SJB200_POINTER_SHARDED_MAX_POINTERS pointers or is over a limit of sjb200_at_pointer_dev, or the stream has 2^32 - 3
+ * structurals or more; UNEXPECTED_ERROR when a peer enqueued another kind for the pass, when a rank could not run its
+ * pass, when the ranks disagree on whole or on the pointers (their count and a 64-bit hash of the compiled pointers), or
+ * for a bad table; else SUCCESS.  Rounds: the edge round, then one round per step of the walks (the first step is the
+ * local walks) until a step hands nothing over -- at most nranks of them, one when no walk crosses a cut.  The window
+ * area is DESIGN.md section 5. */
+#define SJB200_POINTER_SHARDED_MAX_POINTERS 1024   /* pointers per sharded call (window space) */
+typedef struct {
+  int32_t error;     /* simdjson::error_code */
+  uint32_t reserved;
+  uint64_t index;    /* global structural index of the selected value / of the first token in error; UINT64_MAX: none */
+} sjb200_sharded_pointer_result;
+typedef struct {
+  int error;                 /* as returned */
+  uint32_t rounds;           /* continuation steps this pass ran (0 when no walk crossed a cut) */
+  uint64_t docs_before;      /* documents starting on earlier ranks: d_out[p * ndocs + j] here is document docs_before + j */
+  uint64_t tokens_before;    /* structurals of earlier ranks */
+  uint64_t ndocs;            /* documents of the stream (whole mode: 1) */
+  uint64_t walks_forwarded;  /* (document, pointer) walks this rank handed to a later rank */
+} sjb200_sharded_pointer_summary;
+SJB200_API int sjb200_at_pointer_sharded_enqueue(sjb200_comm *comm, const uint8_t *d_type, const uint64_t *d_payload, uint32_t n, const uint8_t *d_strbuf,
+                                                 size_t string_bytes, int whole, const sjb200_doc_boundary *d_docs, uint32_t ndocs,
+                                                 const char *const *pointers, const size_t *pointer_lens, int npointers,
+                                                 sjb200_sharded_pointer_result *d_out, void *stream);
+SJB200_API int sjb200_at_pointer_sharded_finish(sjb200_comm *comm, sjb200_sharded_pointer_summary *out);
+SJB200_API int sjb200_at_pointer_sharded(sjb200_comm *comm, const uint8_t *d_type, const uint64_t *d_payload, uint32_t n, const uint8_t *d_strbuf,
+                                         size_t string_bytes, int whole, const sjb200_doc_boundary *d_docs, uint32_t ndocs, const char *const *pointers,
+                                         const size_t *pointer_lens, int npointers, sjb200_sharded_pointer_result *d_out,
+                                         sjb200_sharded_pointer_summary *out, void *stream);
+
 /* the document starts of one shard of a sharded stream pass: (local structural index, shard-relative byte) pairs of
  * d_idx[0, kept), structural 0 counted when first_starts_document says so (both from the pass's result).  A rank's
  * global document numbers are its table's positions plus the other ranks' ndocs before it.  Not collective.
@@ -608,6 +655,43 @@ typedef struct {
  * of rank r's last document (ranks that own none: unchanged).  Returns out->error. */
 SJB200_API int sjb200_grammar_result_fold(int nranks, const sjb200_grammar_edge *edges, const sjb200_grammar_tally *tallies,
                                           sjb200_sharded_document_errors_result *out, sjb200_sharded_document_error *last /* nranks */);
+
+/* the host fold of a sharded pointer pass's edge round, pure: what every rank's finish computes.  Per rank: */
+typedef struct {
+  uint32_t n;            /* structurals */
+  uint32_t ndocs;        /* table entries (whole mode: 0) */
+  uint32_t flags;        /* bit0 the rank could not run its pass, bit1 bad table, bit2 whole, bit3 over a limit */
+  uint32_t npointers;
+  uint64_t hash;         /* of the compiled pointers */
+  uint32_t types;        /* types of structurals 0 and n - 1, a byte each from the low one (0xFF: none) */
+  uint32_t first_entry;  /* the table's first entry (n without one): structurals before it are the leading segment */
+  uint32_t lead_error_index;  /* local index of the first token in error of the leading segment (0xFFFFFFFF: none) */
+  uint32_t lead_error;        /* its error code */
+} sjb200_pointer_edge;
+typedef struct {
+  uint64_t tokens_before;
+  uint64_t docs_before;
+  uint32_t owned;            /* results this rank writes: its table's documents (whole mode: 1 on rank 0) */
+  uint32_t walks;            /* documents whose walks start here: owned, but in whole mode 1 on the first rank with n > 0 */
+  int32_t prev_holder;       /* the last earlier rank with n > 0 (-1: none): it hands walks to this rank */
+  int32_t next_holder;       /* the next later rank with n > 0 (-1: none) */
+  uint32_t next_type;        /* type of the structural after this rank's last (0xFF: none) */
+  int32_t lead_owner;        /* the rank whose document this rank's leading segment continues (-1: none) */
+  int32_t tail_owner;        /* the rank whose document holds this rank's last structural (-1: none) */
+  uint32_t tail_continues;   /* that document goes on past this rank */
+  int32_t tail_through;      /* the last rank it reaches */
+  uint32_t tail_error;       /* the first token in error of its pieces on later ranks (0: none) */
+  uint64_t tail_after;       /* its structurals on later ranks */
+  uint64_t tail_error_index; /* global index of that token (UINT64_MAX: none) */
+} sjb200_pointer_rank;
+typedef struct {
+  int error;             /* SUCCESS, CAPACITY or UNEXPECTED_ERROR (a failed rank, whole / pointers disagree) */
+  uint32_t bad_table;    /* some rank's table is bad (whole = 0; the pass then fails after writing its results) */
+  uint64_t n;            /* structurals of the stream */
+  uint64_t ndocs;        /* documents of the stream */
+} sjb200_pointer_edge_fold_result;
+SJB200_API int sjb200_pointer_edge_fold(int nranks, const sjb200_pointer_edge *edges, sjb200_pointer_edge_fold_result *res,
+                                        sjb200_pointer_rank *ranks /* nranks */);
 
 /* fold: state entering shard r given the ttables of shards 0..r-1 and the document's initial state 0 */
 SJB200_API uint32_t sjb200_fold_state(const uint32_t *ttables, int nshards_before);

@@ -31,6 +31,7 @@ EXPORTS = [
     "sjb200_at_pointer_dev", "sjb200_document_errors_dev",
     "sjb200_document_errors_sharded", "sjb200_document_errors_sharded_enqueue", "sjb200_document_errors_sharded_finish",
     "sjb200_grammar_edge_fold", "sjb200_grammar_result_fold",
+    "sjb200_at_pointer_sharded", "sjb200_at_pointer_sharded_enqueue", "sjb200_at_pointer_sharded_finish", "sjb200_pointer_edge_fold",
 ]
 COMM_HANDLE_BYTES = 64
 
@@ -149,6 +150,30 @@ class GrammarTally(C.Structure):
     _fields_ = [("lead", C.c_uint64), ("last", C.c_uint64), ("first_key", C.c_uint64), ("errors", C.c_uint32), ("first_doc", C.c_uint32)]
 
 
+class ShardedPointerResult(C.Structure):
+    _fields_ = [("error", C.c_int32), ("reserved", C.c_uint32), ("index", C.c_uint64)]
+
+
+class ShardedPointerSummary(C.Structure):
+    _fields_ = [("error", C.c_int), ("rounds", C.c_uint32), ("docs_before", C.c_uint64), ("tokens_before", C.c_uint64), ("ndocs", C.c_uint64),
+                ("walks_forwarded", C.c_uint64)]
+
+
+class PointerEdge(C.Structure):
+    _fields_ = [("n", C.c_uint32), ("ndocs", C.c_uint32), ("flags", C.c_uint32), ("npointers", C.c_uint32), ("hash", C.c_uint64), ("types", C.c_uint32),
+                ("first_entry", C.c_uint32), ("lead_error_index", C.c_uint32), ("lead_error", C.c_uint32)]
+
+
+class PointerRank(C.Structure):
+    _fields_ = [("tokens_before", C.c_uint64), ("docs_before", C.c_uint64), ("owned", C.c_uint32), ("walks", C.c_uint32), ("prev_holder", C.c_int32),
+                ("next_holder", C.c_int32), ("next_type", C.c_uint32), ("lead_owner", C.c_int32), ("tail_owner", C.c_int32), ("tail_continues", C.c_uint32),
+                ("tail_through", C.c_int32), ("tail_error", C.c_uint32), ("tail_after", C.c_uint64), ("tail_error_index", C.c_uint64)]
+
+
+class PointerEdgeFoldResult(C.Structure):
+    _fields_ = [("error", C.c_int), ("bad_table", C.c_uint32), ("n", C.c_uint64), ("ndocs", C.c_uint64)]
+
+
 def load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
@@ -227,6 +252,11 @@ def load():
         "sjb200_grammar_edge_fold": (C.c_int, [C.c_int, C.POINTER(GrammarEdge), C.POINTER(GrammarEdgeFoldResult), C.POINTER(GrammarRank)]),
         "sjb200_grammar_result_fold": (C.c_int, [C.c_int, C.POINTER(GrammarEdge), C.POINTER(GrammarTally), C.POINTER(ShardedDocumentErrorsResult),
                                                  C.POINTER(ShardedDocumentError)]),
+        "sjb200_at_pointer_sharded": (C.c_int, [vp, vp, vp, C.c_uint32, vp, sz, C.c_int, vp, C.c_uint32, vp, vp, C.c_int, vp,
+                                                C.POINTER(ShardedPointerSummary), vp]),
+        "sjb200_at_pointer_sharded_enqueue": (C.c_int, [vp, vp, vp, C.c_uint32, vp, sz, C.c_int, vp, C.c_uint32, vp, vp, C.c_int, vp, vp]),
+        "sjb200_at_pointer_sharded_finish": (C.c_int, [vp, C.POINTER(ShardedPointerSummary)]),
+        "sjb200_pointer_edge_fold": (C.c_int, [C.c_int, C.POINTER(PointerEdge), C.POINTER(PointerEdgeFoldResult), C.POINTER(PointerRank)]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)

@@ -10,6 +10,7 @@
 #include "sjb200_ctx.h"
 #include "sjb200_grammar.h"
 #include "sjb200_kernels.cuh"
+#include "sjb200_pointer.h"
 
 using namespace sjb200;
 
@@ -98,6 +99,15 @@ struct sjb200_comm {
   } gram[kXchgSteps];
   uint32_t *d_gram_scratch[kXchgSteps] = {};
   size_t gram_scratch_words[kXchgSteps] = {};
+  // pointer passes, by the slot of their pass: the launch (with the compiled pointers' device copy), scratch (grow-only)
+  struct PtrStep {
+    ptr::PtrShard s;
+    bool whole;
+  } ptrs[kXchgSteps];
+  uint8_t *d_ptr_blob[kXchgSteps] = {};
+  size_t ptr_blob_bytes[kXchgSteps] = {};
+  uint32_t *d_ptr_scratch[kXchgSteps] = {};
+  size_t ptr_scratch_words[kXchgSteps] = {};
   cudaStream_t poll_stream = nullptr;
   cudaEvent_t done[kXchgSteps] = {};
   struct Step {
@@ -195,6 +205,8 @@ extern "C" void sjb200_comm_destroy(sjb200_comm *m) {
   cudaFree(m->window); cudaFree(m->d_result); cudaFree(m->d_scratch); cudaFree(m->d_tok_tot);
   for (uint8_t *p : m->d_tok_scratch) cudaFree(p);
   for (uint32_t *p : m->d_gram_scratch) cudaFree(p);
+  for (uint8_t *p : m->d_ptr_blob) cudaFree(p);
+  for (uint32_t *p : m->d_ptr_scratch) cudaFree(p);
   if (m->h_rec) cudaFreeHost(m->h_rec);
   if (m->poll_stream) cudaStreamDestroy(m->poll_stream);
   for (auto e : m->done) if (e) cudaEventDestroy(e);
@@ -841,4 +853,215 @@ extern "C" int sjb200_document_errors_sharded(sjb200_comm *m, const uint8_t *d_t
   int rc = sjb200_document_errors_sharded_enqueue(m, d_type, d_payload, n, whole, d_docs, ndocs, max_depth, d_out, stream);
   if (rc != SJB200_SUCCESS) return rc;
   return sjb200_document_errors_sharded_finish(m, out);
+}
+
+// ---------------------------------------------------------------------------------------------- sharded JSON Pointer
+namespace {
+// FNV-1a over the compiled pointers: the ranks must walk the same ones
+uint64_t blob_hash(const std::vector<uint8_t> &b) {
+  uint64_t h = 0xcbf29ce484222325ull;
+  for (uint8_t c : b) h = (h ^ c) * 0x100000001b3ull;
+  return h;
+}
+
+// wait (host polling, bounded) until `nwords` words from word `first` of every rank's part of the pass's pointer block
+// (stride words apart) carry seq; the block's head (edge and count words) -> comm->h_rec
+int ptr_collect(sjb200_comm *m, uint32_t seq, int first, int stride, int nwords) {
+  sjb200_ctx *c = m->ctx;
+  const unsigned long long *src = m->window + xchg_ptr_at(seq);
+  const auto t0 = std::chrono::steady_clock::now();
+  for (;;) {
+    if (!ok(c, cudaMemcpyAsync(m->h_rec, src, size_t(kPtrHeadWords) * 8, cudaMemcpyDeviceToHost, m->poll_stream), "D2H window") ||
+        !ok(c, cudaStreamSynchronize(m->poll_stream), "sync"))
+      return SJB200_UNEXPECTED_ERROR;
+    c->xchg_polls++;
+    bool all = true;
+    for (int r = 0; r < m->nranks && all; r++)
+      for (int k = 0; k < nwords; k++) all = all && uint32_t(m->h_rec[size_t(first) + size_t(r) * stride + k] >> 32) == seq;
+    if (all) {
+      c->xchg_wait_ms += ms_since(t0);
+      return SJB200_SUCCESS;
+    }
+    if (std::chrono::duration_cast<std::chrono::milliseconds>(std::chrono::steady_clock::now() - t0).count() > m->poll_timeout_ms) {
+      c->last_error = "sharded pointer pass: a peer's words did not arrive";
+      return SJB200_UNEXPECTED_ERROR;
+    }
+  }
+}
+}  // namespace
+
+// Enqueue one pointer pass: the pointers compiled on the host into the slot's device blob, the first token in error of
+// each document and of the leading segment, the table's check, then the edge words and the round-0 record into every
+// rank's window.  The walks wait for finish, which knows where the documents end.  A rank that cannot run its pass (bad
+// arguments, device allocation) or is over a limit still publishes, flagged, so that every rank's finish returns alike.
+extern "C" int sjb200_at_pointer_sharded_enqueue(sjb200_comm *m, const uint8_t *d_type, const uint64_t *d_payload, uint32_t n, const uint8_t *d_strbuf,
+                                                 size_t string_bytes, int whole, const sjb200_doc_boundary *d_docs, uint32_t ndocs,
+                                                 const char *const *pointers, const size_t *pointer_lens, int npointers,
+                                                 sjb200_sharded_pointer_result *d_out, void *stream) {
+  if (!m || !m->connected) return SJB200_UNEXPECTED_ERROR;
+  sjb200_comm::Step *st = pass_begin(m, kPointer, 0, 0, nullptr, 0, nullptr, nullptr, stream);
+  if (!st) return SJB200_CAPACITY;
+  static_assert(sizeof(sjb200_sharded_pointer_result) == sizeof(ptr::ShardPtrResult), "layout");
+  sjb200_ctx *c = m->ctx;
+  DeviceGuard g(c->device);
+  const uint32_t i = m->head % uint32_t(kXchgSteps);
+  if (whole || !d_docs) ndocs = 0;
+  bool failed = npointers < 0 || (npointers && (!pointers || !pointer_lens)) || (n && (!d_type || !d_payload)) || (string_bytes && !d_strbuf) ||
+                (npointers && !d_out && (whole ? m->rank == 0 : ndocs > 0));
+  if (failed) c->last_error = "sharded pointer pass: bad arguments";
+  bool over = npointers > kPtrMaxPointers;
+  ptr::CompiledPointers cp;
+  std::vector<uint8_t> blob;
+  if (!failed && !over) {
+    const int rc = ptr::compile_pointers(pointers, pointer_lens, npointers, &cp);
+    over = rc == SJB200_CAPACITY;
+    failed = rc != SJB200_SUCCESS && !over;
+    if (failed) c->last_error = "sharded pointer pass: a null pointer with a non-zero length";
+  }
+  size_t hb = 0, lb = 0;
+  if (!failed && !over) {
+    hb = cp.headers.size() * sizeof(ptr::PtrHeader);
+    lb = cp.levels.size() * sizeof(ptr::PtrLevel);
+    blob.resize(hb + lb + cp.keys.size() + 1, 0);
+    memcpy(blob.data(), cp.headers.data(), hb);
+    memcpy(blob.data() + hb, cp.levels.data(), lb);
+    memcpy(blob.data() + hb + lb, cp.keys.data(), cp.keys.size());
+  }
+  failed = failed || !grow(c, &m->d_ptr_scratch[i], &m->ptr_scratch_words[i], ptr::shard_scratch_words(ndocs), "cudaMalloc(pointer scratch)") ||
+           (!blob.empty() && !grow(c, &m->d_ptr_blob[i], &m->ptr_blob_bytes[i], blob.size(), "cudaMalloc(pointers)"));
+  ptr::PtrShard &s = m->ptrs[i].s;
+  s = ptr::PtrShard{};
+  m->ptrs[i].whole = whole != 0;
+  const uint8_t *db = m->d_ptr_blob[i];
+  s.a.w = ptr::Walk{d_type, d_payload, d_strbuf, string_bytes, reinterpret_cast<const ptr::PtrLevel *>(db + hb), db + hb + lb};
+  s.a.n = n;
+  s.a.docs = ndocs ? reinterpret_cast<const sjb200_doc_boundary_t *>(d_docs) : nullptr;
+  s.a.ndocs = ndocs;
+  s.a.headers = reinterpret_cast<const ptr::PtrHeader *>(db);
+  s.a.npointers = uint32_t(npointers > 0 ? npointers : 0);
+  s.out = reinterpret_cast<ptr::ShardPtrResult *>(d_out);
+  s.scratch = m->d_ptr_scratch[i];
+  const uint32_t flags = (failed ? uint32_t(kPtrEdgeFailed) : 0u) | (whole ? uint32_t(kPtrEdgeWhole) : 0u) | (over ? uint32_t(kPtrEdgeOver) : 0u);
+  if (failed || over) s.a.npointers = 0;  // (nothing is walked: finish fails on every rank)
+  bool good = blob.empty() || ok(c, cudaMemcpyAsync(m->d_ptr_blob[i], blob.data(), blob.size(), cudaMemcpyHostToDevice, st->stream), "H2D pointers");
+  int launched = 0;
+  good = good && ok(c, ptr::launch_shard_edges(s, flags, failed || over ? 0 : blob_hash(blob), comm_target(m, st->seq, 0), xchg_ptr_at(st->seq), c->sm_count,
+                                               st->stream, &launched), "pointer edges");
+  s.a.npointers = uint32_t(npointers > 0 && npointers <= kPtrMaxPointers ? npointers : 0);
+  c->launches += unsigned(launched);
+  return pass_end(m, good);
+}
+
+// Complete the oldest pass in flight, a pointer pass: round 0 (kind), the edge round and its fold (errors every rank
+// sees alike, the bases, the holders, the tail documents), then the steps: the local walks, and while a step hands walks
+// over, the next holders resume them.  Every step ends with a count round.  The results that came back from later ranks
+// go into d_out last.
+extern "C" int sjb200_at_pointer_sharded_finish(sjb200_comm *m, sjb200_sharded_pointer_summary *out) {
+  if (!m || !out || m->tail == m->head) return SJB200_UNEXPECTED_ERROR;
+  sjb200_ctx *c = m->ctx;
+  DeviceGuard g(c->device);
+  memset(out, 0, sizeof(*out));
+  out->error = SJB200_UNEXPECTED_ERROR;
+  const uint32_t slot = m->tail % uint32_t(kXchgSteps);
+  sjb200_comm::Step st;
+  int rc = pass_pop(m, kPointer, &st);
+  if (rc != SJB200_SUCCESS) return rc;
+  ptr::PtrShard s = m->ptrs[slot].s;
+  const int me = m->rank, R = m->nranks;
+  if ((rc = ptr_collect(m, st.seq, 0, kPtrEdgeWords, kPtrEdgeWords)) != SJB200_SUCCESS) return rc;
+  sjb200_pointer_edge e[kMaxRanks];
+  for (int r = 0; r < R; r++) {
+    const unsigned long long *w = m->h_rec + size_t(r) * kPtrEdgeWords;
+    auto u = [&](int k) { return uint32_t(w[k]); };
+    e[r] = sjb200_pointer_edge{u(0), u(1), u(2), u(3), uint64_t(u(4)) | (uint64_t(u(5)) << 32), u(6), u(7), u(8), u(9)};
+  }
+  sjb200_pointer_edge_fold_result res;
+  sjb200_pointer_rank ranks[kMaxRanks];
+  int err = sjb200_pointer_edge_fold(R, e, &res, ranks);
+  const sjb200_pointer_rank &k = ranks[me];
+  out->docs_before = k.docs_before;
+  out->tokens_before = k.tokens_before;
+  out->ndocs = res.ndocs;
+  cudaStream_t ps = m->poll_stream;
+  if (err != SJB200_SUCCESS) {
+    int failed = -1;
+    for (int r = 0; r < R && failed < 0; r++)
+      if (e[r].flags & kPtrEdgeFailed) failed = r;
+    if (failed >= 0 && failed != me)
+      c->last_error = "sharded pointer pass " + std::to_string(st.seq) + ": rank " + std::to_string(failed) + " could not run its pass";
+    else if (failed < 0 && err == SJB200_UNEXPECTED_ERROR)
+      c->last_error = "sharded pointer pass " + std::to_string(st.seq) + ": the ranks disagree on whole or on the pointers";
+    out->error = err;
+    return err;
+  }
+  s.tokens_before = k.tokens_before;
+  s.owned = k.owned;
+  const uint64_t np = s.a.npointers;
+  if (res.bad_table || (m->ptrs[slot].whole && res.n == 0)) {  // every result {UNEXPECTED_ERROR, none}
+    if (!ok(c, ptr::launch_shard_fill(s.out, np * s.owned, ptr::kUnexpectedError, c->sm_count, ps), "pointer results") || !ok(c, cudaStreamSynchronize(ps), "sync"))
+      return SJB200_UNEXPECTED_ERROR;
+    c->launches += (np && s.owned) ? 1 : 0;
+    if (res.bad_table) c->last_error = "sharded pointer pass: a rank's document table is not strictly ascending or has an entry at or above its n";
+    out->error = res.bad_table ? SJB200_UNEXPECTED_ERROR : SJB200_SUCCESS;
+    return out->error;
+  }
+  out->error = SJB200_SUCCESS;
+  if ((!m->ptrs[slot].whole && res.ndocs == 0) || np == 0) return SJB200_SUCCESS;  // no document on any rank / no pointer
+  const size_t base = xchg_ptr_at(st.seq);
+  auto area = [&](int r, size_t at) { return r < 0 ? nullptr : m->peer[r] + base + at; };
+  s.v = ptr::ShardView{s.a.n, k.next_type, k.tail_continues, uint64_t(s.a.n) + k.tail_after};
+  s.walks = k.walks;
+  s.lead_end = e[me].first_entry;
+  s.tail_err = int32_t(k.tail_error);
+  s.tail_err_index = k.tail_error_index;
+  s.tail_res = k.tail_owner >= 0 && k.tail_owner != me ? area(k.tail_owner, kPtrResAt) : nullptr;
+  s.lead_res = k.lead_owner >= 0 && k.lead_owner != me ? area(k.lead_owner, kPtrResAt) : nullptr;
+  s.seq = st.seq;
+  const Xchg x = comm_target(m, st.seq, 2);
+  // step 0: the local walks; step t > 0: the walks handed over in step t - 1.  A rank writes step t's records into the
+  // next holder's buffer t % 2 only after every rank's count of step t - 1 arrived, and the reader of buffer t % 2
+  // (step t - 2's records) posted that count after its resume: the buffers never overlap in time.
+  uint32_t step = 0;
+  for (;; step++) {
+    s.step = step;
+    s.next_rec = area(k.next_holder, kPtrRecAt + size_t(step & 1u) * kPtrMaxPointers * 2);
+    s.rec_in = m->window + base + kPtrRecAt + size_t((step + 1) & 1u) * kPtrMaxPointers * 2;
+    int launched = 0;
+    if (step == 0) {
+      if (!ok(c, ptr::launch_shard_walks(s, c->sm_count, ps, &launched), "pointer walks")) return SJB200_UNEXPECTED_ERROR;
+    } else if (k.prev_holder >= 0 && uint32_t(m->h_rec[kPtrCountAt + size_t(k.prev_holder) * kMaxRanks + step - 1]) > 0) {
+      const bool cta = s.lead_end > ptr::kCtaMinStructurals;  // (the piece the walks resume over)
+      if (!ok(c, ptr::launch_shard_resume(s, cta, ps), "pointer resume")) return SJB200_UNEXPECTED_ERROR;
+      launched = 1;
+    }
+    if (!ok(c, ptr::launch_shard_post_count(s.scratch, x, base, step, ps), "pointer count")) return SJB200_UNEXPECTED_ERROR;
+    c->launches += unsigned(launched) + 1;
+    if ((rc = ptr_collect(m, st.seq, kPtrCountAt + int(step), kMaxRanks, 1)) != SJB200_SUCCESS) return rc;
+    uint64_t handed = 0;
+    for (int r = 0; r < R; r++) handed += uint32_t(m->h_rec[kPtrCountAt + size_t(r) * kMaxRanks + step]);
+    out->walks_forwarded += uint32_t(m->h_rec[kPtrCountAt + size_t(me) * kMaxRanks + step]);
+    if (handed == 0) break;
+    if (step + 1 >= uint32_t(R)) {  // (a walk crosses each cut at most once)
+      c->last_error = "sharded pointer pass: walks still handed over after every rank";
+      return SJB200_UNEXPECTED_ERROR;
+    }
+  }
+  out->rounds = step;
+  // the results of this rank's document that ended on later ranks
+  const bool gets = s.owned && (m->ptrs[slot].whole ? k.walks == 0 || k.tail_continues : (k.tail_owner == me && k.tail_continues));
+  if (gets && !ok(c, ptr::launch_shard_scatter(m->window + base + kPtrResAt, st.seq, s.out, uint32_t(np), s.owned, ps), "pointer results"))
+    return SJB200_UNEXPECTED_ERROR;
+  c->launches += gets ? 1 : 0;
+  if (!ok(c, cudaStreamSynchronize(ps), "sync")) return SJB200_UNEXPECTED_ERROR;
+  return SJB200_SUCCESS;
+}
+
+extern "C" int sjb200_at_pointer_sharded(sjb200_comm *m, const uint8_t *d_type, const uint64_t *d_payload, uint32_t n, const uint8_t *d_strbuf,
+                                         size_t string_bytes, int whole, const sjb200_doc_boundary *d_docs, uint32_t ndocs, const char *const *pointers,
+                                         const size_t *pointer_lens, int npointers, sjb200_sharded_pointer_result *d_out,
+                                         sjb200_sharded_pointer_summary *out, void *stream) {
+  int rc = sjb200_at_pointer_sharded_enqueue(m, d_type, d_payload, n, d_strbuf, string_bytes, whole, d_docs, ndocs, pointers, pointer_lens, npointers, d_out,
+                                             stream);
+  if (rc != SJB200_SUCCESS) return rc;
+  return sjb200_at_pointer_sharded_finish(m, out);
 }

@@ -374,3 +374,80 @@ extern "C" int sjb200_grammar_result_fold(int nranks, const sjb200_grammar_edge 
   }
   return out->error;
 }
+
+// ---- sharded JSON Pointer lookup (sjb200_at_pointer_sharded)
+// The edge round: every rank's place in the stream, the ranks its walks are handed between, and for the document that
+// holds its last structural (its tail document): whether it goes on past the rank, how many structurals it has on later
+// ranks, and the first token in error of those pieces.  A document's piece on a later rank is that rank's leading
+// segment (all of its structurals when it has no table entry); ranks with 0 structurals hold no piece.  The bases, the
+// ownership and the type after a rank's last structural are the grammar's edge fold.
+extern "C" int sjb200_pointer_edge_fold(int nranks, const sjb200_pointer_edge *e, sjb200_pointer_edge_fold_result *res, sjb200_pointer_rank *ranks) {
+  if (!e || !res || !ranks || nranks < 1 || nranks > kMaxRanks) return SJB200_UNEXPECTED_ERROR;
+  memset(res, 0, sizeof(*res));
+  memset(ranks, 0, sizeof(*ranks) * size_t(nranks));
+  const bool whole = (e[0].flags & kPtrEdgeWhole) != 0;
+  sjb200_grammar_edge ge[kMaxRanks];
+  bool failed = false, over = false, differ = false;
+  for (int r = 0; r < nranks; r++) {
+    failed = failed || (e[r].flags & kPtrEdgeFailed);
+    over = over || (e[r].flags & kPtrEdgeOver) || e[r].npointers > uint32_t(kPtrMaxPointers);
+    differ = differ || ((e[r].flags & kPtrEdgeWhole) != 0) != whole || e[r].npointers != e[0].npointers || e[r].hash != e[0].hash;
+    if (!whole && (e[r].flags & kPtrEdgeBadTable)) res->bad_table = 1;
+    const uint32_t t0 = e[r].types & 0xFFu, t1 = (e[r].types >> 8) & 0xFFu;
+    ge[r] = sjb200_grammar_edge{e[r].n, whole ? 0u : e[r].ndocs, (e[r].flags & kPtrEdgeWhole) ? uint32_t(kGramEdgeWhole) : 0u, 1u,
+                                t0 | 0xFFFF00u | (t1 << 24), e[r].first_entry};
+  }
+  sjb200_grammar_edge_fold_result gres;
+  sjb200_grammar_rank g[kMaxRanks];
+  sjb200_grammar_edge_fold(nranks, ge, &gres, g);
+  over = over || gres.n > 0xFFFFFFFCull;  // kSuspend, kNone and every index a walk reaches must stay apart in 32 bits
+  res->n = gres.n;
+  res->ndocs = gres.ndocs;
+  res->error = failed ? SJB200_UNEXPECTED_ERROR : over ? SJB200_CAPACITY : differ ? SJB200_UNEXPECTED_ERROR : SJB200_SUCCESS;
+  // the leading segment of rank r: [0, lead_end(r)); a table entry at 0 leaves it empty
+  auto lead_end = [&](int r) { return (whole || !e[r].ndocs) ? e[r].n : e[r].first_entry; };
+  int open_owner = -1, prev = -1;  // the owner of the document the structurals so far end in; the last holder
+  for (int r = 0; r < nranks; r++) {
+    sjb200_pointer_rank &k = ranks[r];
+    k.tokens_before = g[r].tokens_before;
+    k.docs_before = g[r].docs_before;
+    k.owned = g[r].owned;
+    k.next_type = g[r].halo_after;
+    k.prev_holder = prev;
+    k.next_holder = -1;
+    for (int q = r + 1; q < nranks && k.next_holder < 0; q++)
+      if (e[q].n) k.next_holder = q;
+    k.lead_owner = k.tail_owner = k.tail_through = -1;
+    k.tail_error_index = ~0ull;
+    if (!e[r].n) continue;
+    if (whole) {
+      k.walks = open_owner < 0 ? 1u : 0u;  // the first holder walks from the root
+      k.lead_owner = open_owner;
+      open_owner = 0;
+    } else {
+      k.walks = e[r].ndocs;
+      k.lead_owner = lead_end(r) > 0 ? open_owner : -1;
+      if (e[r].ndocs) open_owner = r;
+    }
+    k.tail_owner = open_owner;
+    prev = r;
+  }
+  for (int r = 0; r < nranks; r++) {
+    sjb200_pointer_rank &k = ranks[r];
+    if (!e[r].n || k.tail_owner < 0) continue;
+    for (int q = k.next_holder; q >= 0 && q < nranks; q++) {
+      if (!e[q].n) continue;
+      const uint32_t le = lead_end(q);
+      if (le == 0) break;  // a document starts at q's structural 0
+      k.tail_continues = 1;
+      k.tail_through = q;
+      k.tail_after += le;
+      if (!k.tail_error && e[q].lead_error_index != 0xFFFFFFFFu) {
+        k.tail_error = e[q].lead_error;
+        k.tail_error_index = g[q].tokens_before + e[q].lead_error_index;
+      }
+      if (le < e[q].n) break;  // the document ends on q
+    }
+  }
+  return res->error;
+}

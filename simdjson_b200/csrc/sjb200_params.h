@@ -20,8 +20,10 @@ constexpr int kXchgSteps = 64;                        // sharded passes whose ex
 
 // ---- scan kinds (kStream: a stage-1 pass of the sharded streaming modes; kDelim: one of the sharded RS / comma-delimited
 // modes.  Both scan like kIndex, only their records differ.  kTokens: a sharded stage-2-lite pass, whose record comes
-// from tile_scan_kernel, sjb200_tape.cu.  kGrammar: a sharded stage-2 grammar pass, sjb200_grammar.cu)
-enum : int { kIndex = 0, kMinify = 1, kUtf8 = 2, kStream = 3, kDelim = 4, kTokens = 5, kGrammar = 6 };
+// from tile_scan_kernel, sjb200_tape.cu.  kGrammar: a sharded stage-2 grammar pass, sjb200_grammar.cu.  kPointer: a
+// sharded JSON Pointer pass, sjb200_pointer.cu.  kPointer = 7 is the last value the record's 3-bit kind field holds: a
+// further kind needs a wider field)
+enum : int { kIndex = 0, kMinify = 1, kUtf8 = 2, kStream = 3, kDelim = 4, kTokens = 5, kGrammar = 6, kPointer = 7 };
 // a kTokens record's flags: kFlagInternal (the rank could not run its pass), or this rank's string bytes exceed its
 // string buffer (it wrote no records)
 constexpr uint32_t kTokShortFlag = 8u;
@@ -110,7 +112,7 @@ struct ScanParams {
 // one shard record as two independently tagged 64-bit words (8-byte stores are single transactions):
 //   w0 = seq[30:0] << 33 | count[32:0]        w1 = seq << 32 | kind << 24 | flags << 16 | ttable << 8 | state_out
 // kind (3 bits, 24-26) is the scan kind of the pass (kIndex 0, kMinify 1, kUtf8 2, kStream 3, kDelim 4, kTokens 5,
-// kGrammar 6); count is structurals (kIndex, kStream, kDelim, kGrammar: the rank's tokens), kept bytes (kMinify), 0 (kUtf8)
+// kGrammar 6, kPointer 7: the field is full); count is structurals (kIndex, kStream, kDelim, kGrammar: the rank's tokens), kept bytes (kMinify), 0 (kUtf8)
 // or string bytes (kTokens, whose state_out
 // field carries the state the caller says the shard starts in).  Bit 26 was zero before kDelim existed, so the records of
 // the other kinds are unchanged.
@@ -169,9 +171,31 @@ constexpr int kGramWords = 146;
 enum : int { kGramEdgeAt = 0, kGramEdgeWords = 6, kGramRecAt = 8, kGramResAt = 138, kGramResWords = 8 };
 enum : uint32_t { kGramEdgeFailed = 1, kGramEdgeBadTable = 2, kGramEdgeWhole = 4, kGramEdgeFirstStarts = 8, kGramEdgeLastStarts = 16 };
 constexpr size_t kXchgGramWords = size_t(kXchgSteps) * kMaxRanks * kGramWords;
-constexpr size_t kXchgWindowWords = kXchgRecordWords + kXchgSummaryWords + kXchgDelimWords + kXchgGramWords;
 SJ_PARAMS_HD inline size_t xchg_gram_at(uint32_t seq, uint32_t rank) {
   return kXchgRecordWords + kXchgSummaryWords + kXchgDelimWords + (size_t(seq % uint32_t(kXchgSteps)) * kMaxRanks + rank) * kGramWords;
+}
+// A pointer pass's block (sjb200_at_pointer_sharded), kPtrSlotWords words per slot -- one block per window, not per rank:
+// at most one document crosses each rank's end, so a rank receives the walks of at most one document and returns the
+// results of at most one (kPtrMaxPointers each).
+//   edge round    [kMaxRanks][kPtrEdgeWords], each seq << 32 | payload: 0 n   1 ndocs   2 kPtrEdge* bits   3 npointers
+//                 4 / 5 low / high half of the pointer set's hash   6 types of structurals 0 and n - 1 (a byte each, 0xFF:
+//                 none)   7 the
+//                 table's first entry (n without one)   8 local index of the first token in error before it
+//                 (0xFFFFFFFF: none)   9 its error code
+//   count rounds  [kMaxRanks][kMaxRanks]: [rank][step] seq << 32 | walks the rank handed over in that step
+//   records       [2][kPtrMaxPointers][2]: the walks handed to this rank, by pointer, double-buffered by step parity
+//                 (sjb200_pointer.cuh pack_walk)
+//   results       [kPtrMaxPointers][2]: seq << 32 | error, global index -- the walks of this rank's document that ended
+//                 on later ranks, by pointer
+constexpr int kPtrMaxPointers = 1024;  // SJB200_POINTER_SHARDED_MAX_POINTERS
+constexpr int kPtrEdgeWords = 10;
+enum : int { kPtrCountAt = kMaxRanks * kPtrEdgeWords, kPtrHeadWords = kPtrCountAt + kMaxRanks * kMaxRanks, kPtrRecAt = kPtrHeadWords,
+             kPtrResAt = kPtrRecAt + 2 * kPtrMaxPointers * 2, kPtrSlotWords = kPtrResAt + kPtrMaxPointers * 2 };
+enum : uint32_t { kPtrEdgeFailed = 1, kPtrEdgeBadTable = 2, kPtrEdgeWhole = 4, kPtrEdgeOver = 8 };
+constexpr size_t kXchgPtrWords = size_t(kXchgSteps) * kPtrSlotWords;
+constexpr size_t kXchgWindowWords = kXchgRecordWords + kXchgSummaryWords + kXchgDelimWords + kXchgGramWords + kXchgPtrWords;
+SJ_PARAMS_HD inline size_t xchg_ptr_at(uint32_t seq) {
+  return kXchgRecordWords + kXchgSummaryWords + kXchgDelimWords + kXchgGramWords + size_t(seq % uint32_t(kXchgSteps)) * kPtrSlotWords;
 }
 
 }  // namespace sjb200

@@ -123,15 +123,50 @@ struct CtaGroup {
   }
 };
 
-// The children of the container whose opening structural is c, searched for the key (object) or index (array) of level
-// l.  Returns the structural index of the selected value, or kNone with *err set.  Structurals at or past `end` are never
-// read; a container that is not closed before it (a document the reference rejects for its nesting) ends the search.
-template <class G, int ITEMS>
-SJ_DEV uint32_t find_child(G &g, const Walk &w, uint32_t c, bool obj, const PtrLevel &l, uint32_t end, int32_t *err) {
-  int depth = 0;        // relative depth entering this step
-  uint32_t ord = 0;     // array elements before this step
-  for (uint64_t pos = uint64_t(c) + 1;; pos += uint64_t(G::kWidth) * ITEMS) {
-    if (pos >= end) break;
+// Where a cut between ranks stops a walk (sjb200_at_pointer_sharded).  NoCut: the unsharded walk, every structural of
+// the document lies in [0, end).  ShardCut: one rank's piece of a document whose structurals go on past this rank's
+// last one when `continues`; the walk then reads nothing at or past `end` (the rank's n), takes the type of the
+// structural after it from the halo, and suspends where the unsharded walk would run into the end.
+struct NoCut {
+  static constexpr bool kSuspends = false;
+  static constexpr uint32_t continues = 0;
+  // is the key string at k followed by its ':' and a value inside the document
+  SJ_DEV bool key_at(const Walk &w, uint64_t k, uint32_t end) const { return k + 2 < end && w.type[k + 1] == ':'; }
+};
+struct ShardCut {
+  static constexpr bool kSuspends = true;
+  uint32_t next_type;  // type of the structural after this rank's last one (the next holder's structural 0)
+  uint32_t continues;  // the document goes on past this rank's last structural
+  uint64_t doc_end;    // the document's end, counted from this rank's structural 0 (end itself when !continues)
+  SJ_DEV bool key_at(const Walk &w, uint64_t k, uint32_t end) const {
+    return k + 2 < doc_end && (k + 1 < end ? uint32_t(w.type[k + 1]) : next_type) == ':';
+  }
+};
+constexpr uint32_t kSuspend = 0xFFFFFFFEu;  // find_child / walk_from: the walk reached the end of a piece inside its document
+
+// a search inside a container: the relative depth and the array elements counted before the next structural
+struct Cursor {
+  int32_t depth;
+  uint32_t ord;
+};
+
+// The children of a container, from structural pos on (its opener + 1, or where a suspended search resumes with *cur),
+// searched for the key (object) or index (array) of level l.  Returns the structural index of the selected value
+// (with a ShardCut possibly past end: a key whose ':' or value lies across the cut), kNone with *err set, or kSuspend
+// with *cur at end.  Structurals at or past `end` are never read; a container that is not closed before it (a document
+// the reference rejects for its nesting) ends the search.
+template <class G, int ITEMS, class C>
+SJ_DEV uint32_t find_child(G &g, const Walk &w, uint64_t pos, bool obj, const PtrLevel &l, uint32_t end, const C &cut, Cursor *cur, int32_t *err) {
+  int depth = cur->depth;  // relative depth entering this step
+  uint32_t ord = cur->ord;  // array elements before this step
+  for (;; pos += uint64_t(G::kWidth) * ITEMS) {
+    if (pos >= end) {
+      if (C::kSuspends && cut.continues) {
+        *cur = Cursor{depth, ord};
+        return kSuspend;
+      }
+      break;
+    }
     const uint64_t k0 = pos + uint64_t(g.rank()) * ITEMS;
     uint32_t t[ITEMS];
     int sum = 0;
@@ -152,7 +187,7 @@ SJ_DEV uint32_t find_child(G &g, const Walk &w, uint32_t c, bool obj, const PtrL
         if (tok_close(t[i])) {
           if (close_at == kNone) close_at = uint32_t(k);
         } else if (obj) {
-          if (hit == kNone && close_at == kNone && t[i] == '"' && k + 2 < end && w.type[k + 1] == ':' && key_equals(w, w.payload[k], l))
+          if (hit == kNone && close_at == kNone && t[i] == '"' && cut.key_at(w, k, end) && key_equals(w, w.payload[k], l))
             hit = uint32_t(k);
         } else if (t[i] != ',' && close_at == kNone) {
           elems++;
@@ -192,36 +227,105 @@ SJ_DEV uint32_t find_child(G &g, const Walk &w, uint32_t c, bool obj, const PtrL
   return kNone;
 }
 
-// One (document, pointer) pair: from the document's root structural, every level of the pointer.  Returns the selected
-// structural index or kNone with *err set.
-template <class G, int ITEMS>
-SJ_DEV uint32_t walk_pointer(G &g, const Walk &w, const PtrHeader &h, uint32_t root, uint32_t end, int32_t *err) {
+// Where a walk of one pointer stands: about to take reference token `level` at the value `pos` (open = 0), or inside
+// that token's container (open = 1, its kind in obj), searching on from structural pos with the relative depth and the
+// array elements counted so far.  A suspended walk's state, relative to the start of the next piece.
+struct WalkAt {
+  uint32_t level;
+  uint32_t pos;
+  int32_t depth;
+  uint32_t ord;
+  uint32_t open;
+  uint32_t obj;
+};
+
+// One (document, pointer) pair from `at` on, every remaining level of the pointer.  Returns the selected structural
+// index, kNone with *err set, or (ShardCut only) kSuspend with *susp: where the walk goes on at the next piece.  With a
+// ShardCut the selected index may lie past end (the value of a key on this rank).
+template <class G, int ITEMS, class C>
+SJ_DEV uint32_t walk_from(G &g, const Walk &w, const PtrHeader &h, WalkAt at, uint32_t end, const C &cut, int32_t *err, WalkAt *susp) {
   *err = 0;
   if (h.error != 0) {
     *err = h.error;
     return kNone;
   }
-  uint32_t v = root;
-  for (uint32_t L = 0; L < h.nlevels; L++) {
+  uint32_t v = at.pos;
+  for (uint32_t L = at.level; L < h.nlevels; L++) {
     const PtrLevel l = w.levels[h.level0 + L];
-    const uint32_t t = w.type[v];
-    const bool obj = t == '{';
-    if (!obj && t != '[') {
-      *err = l.scalar_error;
-      return kNone;
-    }
-    if (obj ? l.key_error != 0 : l.array_error != 0) {
-      *err = obj ? l.key_error : l.array_error;
-      return kNone;
+    bool obj;
+    uint64_t pos;
+    Cursor cur{0, 0};
+    if (C::kSuspends && at.open) {
+      at.open = 0;
+      obj = at.obj != 0;
+      pos = v;
+      cur = Cursor{at.depth, at.ord};
+    } else {
+      if (C::kSuspends && v >= end) {  // the value of this level lies on a later rank
+        *susp = WalkAt{L, v - end, 0, 0, 0, 0};
+        return kSuspend;
+      }
+      const uint32_t t = w.type[v];
+      obj = t == '{';
+      if (!obj && t != '[') {
+        *err = l.scalar_error;
+        return kNone;
+      }
+      if (obj ? l.key_error != 0 : l.array_error != 0) {
+        *err = obj ? l.key_error : l.array_error;
+        return kNone;
+      }
+      pos = uint64_t(v) + 1;
     }
     int32_t e = 0;
-    v = find_child<G, ITEMS>(g, w, v, obj, l, end, &e);
-    if (v == kNone || v >= end) {
+    v = find_child<G, ITEMS>(g, w, pos, obj, l, end, cut, &cur, &e);
+    if (C::kSuspends && v == kSuspend) {
+      *susp = WalkAt{L, 0, cur.depth, cur.ord, 1, obj ? 1u : 0u};
+      return kSuspend;
+    }
+    if (v == kNone || (!C::kSuspends && v >= end)) {
       *err = e ? e : (obj ? kNoSuchField : kIndexOutOfBounds);
       return kNone;
     }
   }
   return v;
+}
+
+// One (document, pointer) pair: from the document's root structural, every level of the pointer.  Returns the selected
+// structural index or kNone with *err set.
+template <class G, int ITEMS>
+SJ_DEV uint32_t walk_pointer(G &g, const Walk &w, const PtrHeader &h, uint32_t root, uint32_t end, int32_t *err) {
+  WalkAt susp;
+  return walk_from<G, ITEMS>(g, w, h, WalkAt{0, root, 0, 0, 0, 0}, end, NoCut{}, err, &susp);
+}
+
+// One rank's view of the document that holds its last structural (sjb200_at_pointer_sharded; sjb200_pointer_edge_fold).
+struct ShardView {
+  uint32_t n;               // this rank's structurals
+  uint32_t next_type;       // type of the structural after its last one (0xFF: none)
+  uint32_t tail_continues;  // the document holding structural n - 1 goes on past this rank
+  uint64_t tail_end;        // n + that document's structurals on later ranks
+};
+// the cut of a piece [.., end) of this rank's structurals: a piece that ends at n belongs to the document holding n - 1
+SJ_DEV ShardCut piece_cut(const ShardView &v, uint32_t end) {
+  const bool c = v.tail_continues != 0 && end == v.n;
+  return ShardCut{v.next_type, c ? 1u : 0u, c ? v.tail_end : uint64_t(end)};
+}
+
+// A suspended walk as the 16-byte record a rank hands to the next holder of its document (sjb200_at_pointer_sharded):
+//   w0 = seq << 32 | step << 24 | obj << 18 | open << 17 | pos << 16 | level     w1 = ord << 32 | depth
+// pos is 0 or 1 (a value right after the cut, or after its ':'); step tells the double-buffered rounds apart.
+SJ_DEV void pack_walk(const WalkAt &a, uint32_t seq, uint32_t step, unsigned long long *w0, unsigned long long *w1) {
+  *w0 = (static_cast<unsigned long long>(seq) << 32) | (static_cast<unsigned long long>(step & 0xFFu) << 24) |
+        (static_cast<unsigned long long>(a.obj & 1u) << 18) | (static_cast<unsigned long long>(a.open & 1u) << 17) |
+        (static_cast<unsigned long long>(a.pos & 1u) << 16) | (a.level & 0xFFFFu);
+  *w1 = (static_cast<unsigned long long>(a.ord) << 32) | uint32_t(a.depth);
+}
+// false: the record is not of (seq, step) -- no walk of this pointer was handed over in that step
+SJ_DEV bool unpack_walk(unsigned long long w0, unsigned long long w1, uint32_t seq, uint32_t step, WalkAt *a) {
+  if (uint32_t(w0 >> 32) != seq || uint32_t(w0 >> 24 & 0xFFu) != (step & 0xFFu)) return false;
+  *a = WalkAt{uint32_t(w0 & 0xFFFFu), uint32_t(w0 >> 16) & 1u, int32_t(uint32_t(w1)), uint32_t(w1 >> 32), uint32_t(w0 >> 17) & 1u, uint32_t(w0 >> 18) & 1u};
+  return true;
 }
 
 // ---- host: the pointers of one call compiled into one blob [PtrHeader x np][PtrLevel x levels][key bytes], so that

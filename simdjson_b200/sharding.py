@@ -101,6 +101,7 @@ class Comm:
         self.parser, self.rank, self.world = parser, rank, world
         self._tokens_out = collections.deque()  # the outputs of the tokens passes in flight, oldest first
         self._grammar_out = collections.deque()  # ... and of the grammar passes
+        self._pointer_out = collections.deque()  # ... and of the pointer passes
         self._h = C.c_void_p()
         rc = _lib().sjb200_comm_create(parser._ctx, rank, world, C.byref(self._h))
         if rc != 0:
@@ -308,6 +309,64 @@ class Comm:
         if rc != 0:
             return rc, None, None, None
         return self.document_errors_finish()
+
+    # JSON Pointer lookup over this shard's tokens; its passes share the window with the other kinds
+    def at_pointer_enqueue(self, pointers, d_type, d_payload, n, d_strbuf, string_bytes, whole, table=None, stream=None):
+        """pointers: str or bytes, the same on every rank.  (d_type, d_payload, n, d_strbuf, string_bytes): this rank's
+        output of a sharded tokens pass.  whole = True: the ranks hold one document; else table is this rank's document
+        table (as for document_errors_enqueue).  Allocates d_out (npointers x the documents that start here, 16 bytes
+        each) and keeps it until at_pointer_finish returns it."""
+        import torch
+
+        from .implementation import _stream_ptr
+        n = int(n)
+        dev = d_type.device
+        d_docs, ndocs = self._device_table(table, whole, dev)
+        enc = [p.encode() if isinstance(p, str) else bytes(p) for p in pointers]
+        P = len(enc)
+        bufs = [C.create_string_buffer(e, len(e)) for e in enc]
+        ptrs = (C.c_void_p * max(P, 1))(*[C.addressof(b) for b in bufs])
+        lens = (C.c_size_t * max(P, 1))(*[len(e) for e in enc])
+        nout = 1 if whole else ndocs
+        d_out = torch.empty(max(P * nout, 1) * 2, dtype=torch.int64, device=dev)
+        rc = _lib().sjb200_at_pointer_sharded_enqueue(self._h, d_type.data_ptr() if n else None, d_payload.data_ptr() if n else None, n,
+                                                      d_strbuf.data_ptr() if string_bytes else None, int(string_bytes), int(bool(whole)),
+                                                      d_docs.data_ptr() if ndocs else None, ndocs, ptrs, lens, P, d_out.data_ptr(), _stream_ptr(stream))
+        if rc == 0:
+            self._pointer_out.append((d_out, d_docs, P, nout if (not whole or self.rank == 0) else 0))
+        return rc
+
+    def at_pointer_finish(self):
+        """(error_code, ShardedPointerSummary, errors int32[P, k], indexes uint64[P, k]) of the oldest pass in flight: the
+        results of every pointer in the k documents that start on this rank (whole mode: rank 0's one), global structural
+        indexes (UINT64_MAX: none)"""
+        res = self._capi.ShardedPointerSummary()
+        rc = _lib().sjb200_at_pointer_sharded_finish(self._h, C.byref(res))
+        if rc == self._capi.UNEXPECTED_ERROR and "oldest pass in flight is of another kind" in self.parser.last_cuda_error():
+            return rc, res, None, None
+        d_out, _, P, k = self._pointer_out.popleft() if self._pointer_out else (None, None, 0, 0)
+        # d_out holds results on success, and after a bad table (every result UNEXPECTED_ERROR); else nothing was written
+        written = rc == 0 or (rc == self._capi.UNEXPECTED_ERROR and "document table is not strictly ascending" in self.parser.last_cuda_error())
+        if d_out is None or not written or res.ndocs == 0:
+            return rc, res, np.zeros((P, 0), dtype=np.int32), np.zeros((P, 0), dtype=np.uint64)
+        out = d_out[: 2 * P * k].cpu().numpy().view(np.uint64).reshape(P, k, 2)
+        return rc, res, (out[:, :, 0] & 0xFFFFFFFF).astype(np.uint32).view(np.int32), out[:, :, 1].copy()
+
+    def at_pointer(self, pointers, d_type, d_payload, n, d_strbuf, string_bytes, whole, table=None, stream=None):
+        rc = self.at_pointer_enqueue(pointers, d_type, d_payload, n, d_strbuf, string_bytes, whole, table, stream)
+        if rc != 0:
+            return rc, None, None, None
+        return self.at_pointer_finish()
+
+    def _device_table(self, table, whole, dev):
+        """(device tensor of sjb200_doc_boundary or None, entries) from a [ndocs, 2] array or a device tensor"""
+        import torch
+        if whole or table is None or not len(table):
+            return None, 0
+        if isinstance(table, torch.Tensor) and table.is_cuda:
+            return table, table.numel() * table.element_size() // 8
+        arr = np.ascontiguousarray(np.asarray(table, dtype=np.int64).reshape(-1, 2).astype(np.uint32)).view(np.int32).reshape(-1)
+        return torch.from_numpy(arr.copy()).to(dev), len(arr) // 2
 
     def document_table(self, d_shard, d_idx, result, stream=None):
         """the document starts among this shard's kept structurals (result: a ShardedStreamResult, or the `stream` field of
