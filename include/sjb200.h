@@ -54,6 +54,7 @@ enum {
   SJB200_UNCLOSED_STRING = 15,
   SJB200_UNSUPPORTED_ARCHITECTURE = 16,
   SJB200_INCORRECT_TYPE = 17,
+  SJB200_NUMBER_OUT_OF_RANGE = 18,
   SJB200_INDEX_OUT_OF_BOUNDS = 19,
   SJB200_NO_SUCH_FIELD = 20,
   SJB200_INVALID_JSON_POINTER = 22,
@@ -225,6 +226,55 @@ typedef struct {
 SJB200_API int sjb200_at_pointer_dev(sjb200_ctx *ctx, const uint8_t *d_type, const uint64_t *d_payload, uint32_t n, const uint8_t *d_strbuf,
                                      size_t string_bytes, const sjb200_doc_boundary *d_docs, uint32_t ndocs, const char *const *pointers,
                                      const size_t *pointer_lens, int npointers, sjb200_pointer_result *d_out, void *stream);
+
+/* Typed columns from JSON Pointer results on the device: for every row of d_rows (nrows results of sjb200_at_pointer_dev,
+ * as they are: one pointer's column is d_rows + p * ndocs, and several pointers go in one call), what one DOM getter
+ * returns on the element the row selects.  (d_type, d_payload, n, d_strbuf, string_bytes) is the output of
+ * sjb200_tokens_dev the lookup ran on.  Row r, decided in this order:
+ *   1. a row in error stays in error: d_err[r] = its error, d_row_type[r] = 0, the value 0, the string empty;
+ *   2. an index >= n, or at a token that is not a value (',' ':' '}' ']' or 0), is UNEXPECTED_ERROR with d_row_type 0;
+ *      so is (STRING only, where the record is read) a string whose record [u32 length][bytes][0] does not lie inside
+ *      [0, string_bytes).  Nothing outside [0, n) of the token arrays or [0, string_bytes) of d_strbuf is read;
+ *   3. d_row_type[r] = the tape type char of the value ('{' '[' '"' 'l' 'u' 'd' 't' 'f' 'n'), and d_err[r] / the value
+ *      are the getter's (include/simdjson/dom/element-inl.h):
+ *      INT64        get_int64: 'l' its value; 'u' its value up to INT64_MAX, else NUMBER_OUT_OF_RANGE
+ *      UINT64       get_uint64: 'u' its value; 'l' its value when >= 0, else NUMBER_OUT_OF_RANGE
+ *      BOOL         get_bool: 't' 1, 'f' 0
+ *      STRING       get_string: the exact bytes of the record ("\u0000" kept, no terminator), Arrow large_string layout:
+ *                   d_offsets[0] = 0, row r is d_bytes[d_offsets[r], d_offsets[r + 1]), a row in error has length 0
+ *      ARRAY_SIZE   get_array().size(): the elements of a '[' (the structurals at its depth other than ',')
+ *      OBJECT_SIZE  get_object().size(): the fields of a '{' (its strings followed by ':'; duplicate keys count)
+ *      Sizes saturate at 0xFFFFFF like the tape's scope count (src/generic/stage2/tape_builder.h, cntsat).  Any other
+ *      type is INCORRECT_TYPE; a 'd' value (a float, not converted on the device) is INCORRECT_TYPE under INT64 / UINT64
+ *      as in the reference, and its row type tells it apart.  On an error the value is 0.
+ * d_values: nrows uint64 (INT64: the int64 bits; UINT64; the sizes) or nrows uint8 (BOOL); not used for STRING.  d_offsets
+ * (nrows + 1 int64) and d_bytes (bytes_capacity bytes) are used by STRING only.  Outputs are device memory and stay there;
+ * nothing outside the rows and no byte of d_bytes past out->string_bytes is written.  The call synchronises its stream
+ * once.  Its device scratch (kept by the context) is about 30 bytes per row, plus for STRING bytes_capacity / 512.  nrows = 0 writes d_offsets[0] = 0 (STRING) and nothing else.
+ * Deviations: the rows carry no document end, so a size walk stops at n -- a container the reference rejects for its
+ * nesting is counted up to there, never a fault (as for sjb200_at_pointer_dev); 1e400 and other infinite floats are 'd'
+ * rows here where the reference fails the parse.
+ * Returns SUCCESS; CAPACITY for STRING when bytes_capacity is less than the column's bytes (d_err, d_row_type and
+ * d_offsets are written, nothing to d_bytes, out->string_bytes holds the need -- the contract of sjb200_tokens_dev's
+ * d_strbuf); UNEXPECTED_ERROR for an unknown kind or a NULL output the kind needs; MEMALLOC or UNEXPECTED_ERROR for a
+ * CUDA failure. */
+enum {
+  SJB200_COLUMN_INT64 = 1,        /* element::get_int64            -> int64_t  values */
+  SJB200_COLUMN_UINT64 = 2,       /* element::get_uint64           -> uint64_t values */
+  SJB200_COLUMN_BOOL = 3,         /* element::get_bool             -> uint8_t  values (0 / 1) */
+  SJB200_COLUMN_STRING = 4,       /* element::get_string           -> int64 offsets[nrows + 1] + bytes */
+  SJB200_COLUMN_ARRAY_SIZE = 5,   /* element::get_array().size()   -> uint64_t values */
+  SJB200_COLUMN_OBJECT_SIZE = 6   /* element::get_object().size()  -> uint64_t values */
+};
+typedef struct {
+  uint32_t rows_in_error;
+  uint32_t reserved;
+  uint64_t string_bytes;          /* STRING: bytes of the packed column (under CAPACITY: the bytes needed) */
+} sjb200_column_result;
+SJB200_API int sjb200_column_dev(sjb200_ctx *ctx, int kind, const uint8_t *d_type, const uint64_t *d_payload, uint32_t n, const uint8_t *d_strbuf,
+                                 size_t string_bytes, const sjb200_pointer_result *d_rows, uint32_t nrows, int32_t *d_err, uint8_t *d_row_type,
+                                 void *d_values, int64_t *d_offsets, uint8_t *d_bytes, size_t bytes_capacity, sjb200_column_result *out,
+                                 void *stream);
 
 /* Stage-2 grammar on the device: for every document, the error json_iterator::walk_document
  * (src/generic/stage2/json_iterator.h L120-244, with tape_builder) returns, from the output of sjb200_tokens_dev (d_type,

@@ -32,6 +32,7 @@ EXPORTS = [
     "sjb200_document_errors_sharded", "sjb200_document_errors_sharded_enqueue", "sjb200_document_errors_sharded_finish",
     "sjb200_grammar_edge_fold", "sjb200_grammar_result_fold",
     "sjb200_at_pointer_sharded", "sjb200_at_pointer_sharded_enqueue", "sjb200_at_pointer_sharded_finish", "sjb200_pointer_edge_fold",
+    "sjb200_column_dev",
 ]
 COMM_HANDLE_BYTES = 64
 
@@ -39,9 +40,12 @@ COMM_HANDLE_BYTES = 64
 SUCCESS, CAPACITY, MEMALLOC, UTF8_ERROR, EMPTY, UNESCAPED_CHARS, UNCLOSED_STRING, UNSUPPORTED_ARCHITECTURE, UNEXPECTED_ERROR = 0, 1, 2, 11, 13, 14, 15, 16, 24
 ERROR_NAMES = {0: "SUCCESS", 1: "CAPACITY", 2: "MEMALLOC", 3: "TAPE_ERROR", 4: "DEPTH_ERROR", 5: "STRING_ERROR", 6: "T_ATOM_ERROR", 7: "F_ATOM_ERROR", 8: "N_ATOM_ERROR",
                9: "NUMBER_ERROR", 10: "BIGINT_ERROR", 11: "UTF8_ERROR", 13: "EMPTY", 14: "UNESCAPED_CHARS", 15: "UNCLOSED_STRING",
-               16: "UNSUPPORTED_ARCHITECTURE", 17: "INCORRECT_TYPE", 19: "INDEX_OUT_OF_BOUNDS", 20: "NO_SUCH_FIELD", 22: "INVALID_JSON_POINTER",
+               16: "UNSUPPORTED_ARCHITECTURE", 17: "INCORRECT_TYPE", 18: "NUMBER_OUT_OF_RANGE", 19: "INDEX_OUT_OF_BOUNDS", 20: "NO_SUCH_FIELD", 22: "INVALID_JSON_POINTER",
                24: "UNEXPECTED_ERROR"}
 INCORRECT_TYPE, INDEX_OUT_OF_BOUNDS, NO_SUCH_FIELD, INVALID_JSON_POINTER = 17, 19, 20, 22
+NUMBER_OUT_OF_RANGE = 18
+# kinds of sjb200_column_dev (SJB200_COLUMN_*)
+COLUMN_INT64, COLUMN_UINT64, COLUMN_BOOL, COLUMN_STRING, COLUMN_ARRAY_SIZE, COLUMN_OBJECT_SIZE = 1, 2, 3, 4, 5, 6
 DEPTH_ERROR = 4
 # the deepest max_depth sjb200_document_errors_dev accepts (SJB200_DOCUMENT_MAX_DEPTH)
 DOCUMENT_MAX_DEPTH = 4096
@@ -118,6 +122,10 @@ class ShardedTokensResult(C.Structure):
 
 class PointerResult(C.Structure):
     _fields_ = [("error", C.c_int32), ("index", C.c_uint32)]
+
+
+class ColumnResult(C.Structure):
+    _fields_ = [("rows_in_error", C.c_uint32), ("reserved", C.c_uint32), ("string_bytes", C.c_uint64)]
 
 
 class DocumentErrorsResult(C.Structure):
@@ -257,6 +265,7 @@ def load():
         "sjb200_at_pointer_sharded_enqueue": (C.c_int, [vp, vp, vp, C.c_uint32, vp, sz, C.c_int, vp, C.c_uint32, vp, vp, C.c_int, vp, vp]),
         "sjb200_at_pointer_sharded_finish": (C.c_int, [vp, C.POINTER(ShardedPointerSummary)]),
         "sjb200_pointer_edge_fold": (C.c_int, [C.c_int, C.POINTER(PointerEdge), C.POINTER(PointerEdgeFoldResult), C.POINTER(PointerRank)]),
+        "sjb200_column_dev": (C.c_int, [vp, C.c_int, vp, vp, C.c_uint32, vp, sz, vp, C.c_uint32, vp, vp, vp, vp, vp, sz, C.POINTER(ColumnResult), vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)

@@ -10,6 +10,7 @@
 #include <new>
 
 #include "sjb200_bits.cuh"
+#include "sjb200_column.h"
 #include "sjb200_ctx.h"  // (with the CUDA runtime, include/sjb200.h and the launchers of sjb200_docs.cu and sjb200_tape.cu)
 #include "sjb200_finish.h"
 #include "sjb200_hostpipe.h"
@@ -298,7 +299,7 @@ extern "C" void sjb200_destroy(sjb200_ctx *c) {
   if (c->stream) cudaStreamSynchronize(c->stream);
   free_sized(c);
   cudaFree(c->d_carry); cudaFree(c->d_flags); cudaFree(c->d_ticket); cudaFree(c->d_sfin); cudaFree(c->d_doc_scratch); cudaFree(c->d_ndocs); cudaFree(c->d_tok_scratch); cudaFree(c->d_tok_tot); cudaFree(c->d_tails); cudaFree(c->d_debug); cudaFree(c->d_doctab); cudaFree(c->d_stamps);
-  cudaFree(c->d_ptr_blob); cudaFree(c->d_ptr_scratch); cudaFree(c->d_gram_scratch);
+  cudaFree(c->d_ptr_blob); cudaFree(c->d_ptr_scratch); cudaFree(c->d_gram_scratch); cudaFree(c->d_col_scratch);
   if (c->h_ptr_blob) cudaFreeHost(c->h_ptr_blob);
   if (c->h_doctab) cudaFreeHost(c->h_doctab);
   if (c->h_carry) cudaFreeHost(c->h_carry);
@@ -849,6 +850,45 @@ extern "C" int sjb200_at_pointer_dev(sjb200_ctx *c, const uint8_t *d_type, const
     return SJB200_UNEXPECTED_ERROR;
   c->launches += 3;
   return SJB200_SUCCESS;
+}
+
+// Typed columns from JSON Pointer results (element::get_int64 / get_uint64 / get_bool / get_string and container sizes
+// of every row) -- sjb200_column.cu
+extern "C" int sjb200_column_dev(sjb200_ctx *c, int kind, const uint8_t *d_type, const uint64_t *d_payload, uint32_t n, const uint8_t *d_strbuf,
+                                 size_t string_bytes, const sjb200_pointer_result *d_rows, uint32_t nrows, int32_t *d_err, uint8_t *d_row_type,
+                                 void *d_values, int64_t *d_offsets, uint8_t *d_bytes, size_t bytes_capacity, sjb200_column_result *out, void *stream) {
+  if (!c || !out || kind < SJB200_COLUMN_INT64 || kind > SJB200_COLUMN_OBJECT_SIZE) return SJB200_UNEXPECTED_ERROR;
+  out->rows_in_error = 0;
+  out->reserved = 0;
+  out->string_bytes = 0;
+  const bool str = kind == SJB200_COLUMN_STRING;
+  if ((n && (!d_type || !d_payload)) || (string_bytes && !d_strbuf) || (str && !d_offsets) ||
+      (nrows && (!d_rows || !d_err || !d_row_type || (!str && !d_values))) || (str && bytes_capacity && !d_bytes))
+    return SJB200_UNEXPECTED_ERROR;
+  static_assert(sizeof(sjb200_pointer_result) == sizeof(col::Row), "layout");
+  DeviceGuard g(c->device);
+  cudaStream_t s = stream_of(c, stream);
+  if (!grow(c, &c->d_col_scratch, &c->col_scratch_words, (col::column_scratch_bytes(nrows, str ? bytes_capacity : 0) + 7) / 8, "cudaMalloc(column scratch)")) return SJB200_MEMALLOC;
+  col::ColLaunch a{};
+  a.c = col::Cols{d_type, d_payload, n, d_strbuf, string_bytes, reinterpret_cast<const col::Row *>(d_rows), nrows};
+  a.kind = kind;
+  a.err = d_err;
+  a.row_type = d_row_type;
+  a.values = d_values;
+  a.offsets = d_offsets;
+  a.bytes = d_bytes;
+  a.bytes_capacity = str ? bytes_capacity : 0;
+  TokenTotals *tot = nullptr;
+  int launches = 0;
+  if (!ok(c, col::launch_column(a, c->d_col_scratch, &tot, c->sm_count, s, &launches), "column") ||
+      !ok(c, cudaMemcpyAsync(c->h_small, tot, sizeof(TokenTotals), cudaMemcpyDeviceToHost, s), "D2H column totals") || !ok(c, cudaStreamSynchronize(s), "sync"))
+    return SJB200_UNEXPECTED_ERROR;
+  c->launches += launches;
+  TokenTotals t;
+  memcpy(&t, c->h_small, sizeof(t));
+  out->rows_in_error = t.n_strings;
+  if (str) out->string_bytes = t.string_bytes;
+  return str && t.string_bytes > bytes_capacity ? SJB200_CAPACITY : SJB200_SUCCESS;
 }
 
 // Stage-2 grammar over the stage-2-lite tokens (the error walk_document returns for every document) -- sjb200_grammar.cu

@@ -73,6 +73,7 @@ struct sjb200_ctx {
   uint8_t *h_ptr_blob = nullptr; uint8_t *d_ptr_blob = nullptr; size_t ptr_blob_bytes = 0;
   uint32_t *d_ptr_scratch = nullptr; size_t ptr_scratch_words = 0;
   uint32_t *d_gram_scratch = nullptr; size_t gram_scratch_words = 0;  // stage-2 grammar (sjb200_grammar.cu)
+  uint64_t *d_col_scratch = nullptr; size_t col_scratch_words = 0;     // typed columns (sjb200_column.cu)
   int grid_u = 0;
   // pinned host mirrors
   sjb200::Carry *h_carry = nullptr;     // [kCarrySlots]

@@ -294,6 +294,11 @@ size_t tokens_scratch_bytes(uint32_t n) {
   return tiles * (sizeof(unsigned long long) + sizeof(uint32_t)) + 64;
 }
 
+cudaError_t launch_tile_scan(unsigned long long *tile_sums, const uint32_t *tile_counts, uint32_t ntiles, TokenTotals *tot, cudaStream_t stream) {
+  tile_scan_kernel<<<1, 1024, 0, stream>>>(tile_sums, tile_counts, ntiles, tot, TokXchg{});
+  return cudaGetLastError();
+}
+
 cudaError_t launch_tokens(const uint8_t *buf, uint64_t len, const uint32_t *idx, uint32_t n, uint8_t *type, uint64_t *payload, uint8_t *strbuf,
                           uint64_t strbuf_capacity, void *scratch, TokenTotals *tot_dev, int stage, cudaStream_t stream, const TokXchg *xchg) {
   const uint32_t tiles = uint32_t((size_t(n) + kTokThreads - 1) / kTokThreads);

@@ -26,6 +26,10 @@ struct TokXchg {
   uint64_t capacity;   // this rank's string buffer
 };
 
+// tile_scan_kernel, the scan of the tokens' tile sums, for another per-tile quantity (sjb200_column_dev): tile_sums[ntiles] become
+// their exclusive prefix sums, tot->string_bytes their total and tot->n_strings the total of tile_counts[ntiles].  One CTA.
+cudaError_t launch_tile_scan(unsigned long long *tile_sums, const uint32_t *tile_counts, uint32_t ntiles, TokenTotals *tot, cudaStream_t stream);
+
 size_t tokens_scratch_bytes(uint32_t n);
 // type[n], payload[n], strbuf[strbuf_capacity]: device memory; scratch: tokens_scratch_bytes(n) bytes, 8-byte aligned;
 // stage: 1 = tiles staged through shared memory (the product path), 0 = every thread reads / writes global memory (kept as

@@ -215,6 +215,55 @@ class dom_parser_implementation:
             raise RuntimeError(f"sjb200_at_pointer_dev: {capi.ERROR_NAMES.get(rc, rc)} {self.last_cuda_error()}")
         return out[:, :D, 0], out[:, :D, 1]
 
+    def column_device(self, kind, d_type, d_payload, d_strbuf, string_bytes, err, idx, stream=None):
+        """one DOM getter (capi.COLUMN_*: get_int64, get_uint64, get_bool, get_string, get_array().size(),
+        get_object().size()) on every row of at_pointer_device's (err, idx), or of one pointer's row of them, on the
+        device (sjb200_column_dev) over the same tokens.  Returns CUDA tensors shaped like err: (error int32, row_type
+        uint8, values) with values int64 (INT64; UINT64 and the sizes as the bits of the uint64) or bool (BOOL); for
+        STRING (error, row_type, offsets int64[rows + 1], bytes uint8[offsets[-1]]), the rows in err's row-major order,
+        row r being bytes[offsets[r]:offsets[r + 1]].  A failure of the call raises."""
+        import torch
+        dev = d_type.device
+        shape = tuple(err.shape)
+        nrows = err.numel()
+        # the {error, index} pairs: the at_pointer_device tensors are views of one (..., 2) int32 tensor, used in place
+        contiguous_pairs = (err.dtype == idx.dtype == torch.int32 and err.shape == idx.shape and err.stride() == idx.stride()
+                            and idx.data_ptr() == err.data_ptr() + 4 and err.is_cuda and idx.is_cuda)
+        if contiguous_pairs:
+            want, acc = [], 2
+            for s in reversed(shape):
+                want.append(acc)
+                acc *= s
+            contiguous_pairs = all(st == w for st, w, s in zip(err.stride(), reversed(want), shape) if s > 1)
+        rows = err if contiguous_pairs else torch.stack((err.to(torch.int32), idx.to(torch.int32)), -1).to(dev)
+        rows_ptr = rows.data_ptr() if nrows else None
+        e = torch.empty(max(nrows, 1), dtype=torch.int32, device=dev)
+        t = torch.empty(max(nrows, 1), dtype=torch.uint8, device=dev)
+        n = d_type.numel()
+        res = capi.ColumnResult()
+
+        def call(values, offsets, d_bytes, cap):
+            return lib().sjb200_column_dev(self._ctx, kind, d_type.data_ptr() if n else None, d_payload.data_ptr() if n else None, n,
+                                           d_strbuf.data_ptr() if string_bytes else None, string_bytes, rows_ptr, nrows, e.data_ptr(), t.data_ptr(),
+                                           values, offsets, d_bytes, cap, C.byref(res), _stream_ptr(stream))
+
+        if kind == capi.COLUMN_STRING:
+            offsets = torch.empty(nrows + 1, dtype=torch.int64, device=dev)
+            rc = call(None, offsets.data_ptr(), None, 0)
+            if rc == capi.CAPACITY:  # the bytes are sized by the first call
+                out_bytes = torch.empty(max(res.string_bytes, 1), dtype=torch.uint8, device=dev)
+                rc = call(None, offsets.data_ptr(), out_bytes.data_ptr(), res.string_bytes)
+            else:
+                out_bytes = torch.empty(1, dtype=torch.uint8, device=dev)
+            if rc != SUCCESS:
+                raise RuntimeError(f"sjb200_column_dev: {capi.ERROR_NAMES.get(rc, rc)} {self.last_cuda_error()}")
+            return e[:nrows].view(shape), t[:nrows].view(shape), offsets, out_bytes[: res.string_bytes]
+        vals = torch.empty(max(nrows, 1), dtype=torch.bool if kind == capi.COLUMN_BOOL else torch.int64, device=dev)
+        rc = call(vals.data_ptr(), None, None, 0)
+        if rc != SUCCESS:
+            raise RuntimeError(f"sjb200_column_dev: {capi.ERROR_NAMES.get(rc, rc)} {self.last_cuda_error()}")
+        return e[:nrows].view(shape), t[:nrows].view(shape), vals[:nrows].view(shape)
+
     def document_errors_device(self, d_type, d_payload, d_docs=None, ndocs=None, max_depth=None, stream=None):
         """the error stage 2 returns for every document (sjb200_document_errors_dev) over the output of tokens_device:
         d_docs = a document table (sjb200_document_table_dev, int32 pairs {index, byte}) and ndocs its entries in use, or
