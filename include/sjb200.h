@@ -245,7 +245,7 @@ SJB200_API int sjb200_at_pointer_dev(sjb200_ctx *ctx, const uint8_t *d_type, con
  *      ARRAY_SIZE   get_array().size(): the elements of a '[' (the structurals at its depth other than ',')
  *      OBJECT_SIZE  get_object().size(): the fields of a '{' (its strings followed by ':'; duplicate keys count)
  *      Sizes saturate at 0xFFFFFF like the tape's scope count (src/generic/stage2/tape_builder.h, cntsat).  Any other
- *      type is INCORRECT_TYPE; a 'd' value (a float, not converted on the device) is INCORRECT_TYPE under INT64 / UINT64
+ *      type is INCORRECT_TYPE; a 'd' value (a float, not converted here: see sjb200_column_double_dev) is INCORRECT_TYPE under INT64 / UINT64
  *      as in the reference, and its row type tells it apart.  On an error the value is 0.
  * d_values: nrows uint64 (INT64: the int64 bits; UINT64; the sizes) or nrows uint8 (BOOL); not used for STRING.  d_offsets
  * (nrows + 1 int64) and d_bytes (bytes_capacity bytes) are used by STRING only.  Outputs are device memory and stay there;
@@ -275,6 +275,31 @@ SJB200_API int sjb200_column_dev(sjb200_ctx *ctx, int kind, const uint8_t *d_typ
                                  size_t string_bytes, const sjb200_pointer_result *d_rows, uint32_t nrows, int32_t *d_err, uint8_t *d_row_type,
                                  void *d_values, int64_t *d_offsets, uint8_t *d_bytes, size_t bytes_capacity, sjb200_column_result *out,
                                  void *stream);
+
+/* Float columns from JSON Pointer results on the device: for every row of d_rows (as for sjb200_column_dev), what
+ * element::get_double returns on the element the row selects, correctly rounded.  (d_buf, len, d_idx) are the input and
+ * the structurals of the stage-1 call, (d_type, d_payload, n) the output of sjb200_tokens_dev on them; a 'd' token k is
+ * the number d_buf[d_idx[k], d_payload[k]).  Row r, decided in this order:
+ *   1. a row in error stays in error: d_err[r] = its error, d_row_type[r] = 0, d_values[r] = +0.0;
+ *   2. an index >= n, at a token that is not a value, or at a 'd' token whose span is empty, not inside [0, len) or not
+ *      a JSON number, is UNEXPECTED_ERROR with d_row_type 0.  Nothing outside [0, n) of the token arrays or [0, len) of
+ *      d_buf is read;
+ *   3. d_row_type[r] = the tape type char of the value, and
+ *      'd'       the binary64 nearest to the number's text (ties to even), as the reference's parse_number writes it;
+ *                NUMBER_ERROR with the value 0 when that is infinite
+ *      'l' 'u'   double(int64) / double(uint64), rounded to nearest even ("-0" is an 'l' 0 and gives +0.0; "-0.0" gives
+ *                -0.0)
+ *      others    INCORRECT_TYPE, the value 0.
+ * Deviation: an infinite float ("1e400") fails the reference's whole parse; here only its row is NUMBER_ERROR (the tokens
+ * already accept it, see sjb200_tokens_dev).  out->rows_in_error counts the rows in error; out->string_bytes is 0.  The
+ * call synchronises its stream once; nothing outside the rows of the outputs is written, and nrows = 0 writes nothing.  A
+ * number of more than 64 bytes is read by a CTA, and one whose value the Eisel-Lemire step leaves open is decided
+ * exactly on its first 768 significant digits (the rest only break ties).  Device scratch (kept by the context): 8
+ * bytes per row.  Returns SUCCESS; UNEXPECTED_ERROR for a NULL output or input that is needed; MEMALLOC or
+ * UNEXPECTED_ERROR for a CUDA failure. */
+SJB200_API int sjb200_column_double_dev(sjb200_ctx *ctx, const uint8_t *d_buf, size_t len, const uint32_t *d_idx, const uint8_t *d_type,
+                                        const uint64_t *d_payload, uint32_t n, const sjb200_pointer_result *d_rows, uint32_t nrows, int32_t *d_err,
+                                        uint8_t *d_row_type, double *d_values, sjb200_column_result *out, void *stream);
 
 /* Stage-2 grammar on the device: for every document, the error json_iterator::walk_document
  * (src/generic/stage2/json_iterator.h L120-244, with tape_builder) returns, from the output of sjb200_tokens_dev (d_type,

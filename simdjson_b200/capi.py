@@ -32,7 +32,7 @@ EXPORTS = [
     "sjb200_document_errors_sharded", "sjb200_document_errors_sharded_enqueue", "sjb200_document_errors_sharded_finish",
     "sjb200_grammar_edge_fold", "sjb200_grammar_result_fold",
     "sjb200_at_pointer_sharded", "sjb200_at_pointer_sharded_enqueue", "sjb200_at_pointer_sharded_finish", "sjb200_pointer_edge_fold",
-    "sjb200_column_dev",
+    "sjb200_column_dev", "sjb200_column_double_dev",
 ]
 COMM_HANDLE_BYTES = 64
 
@@ -44,6 +44,7 @@ ERROR_NAMES = {0: "SUCCESS", 1: "CAPACITY", 2: "MEMALLOC", 3: "TAPE_ERROR", 4: "
                24: "UNEXPECTED_ERROR"}
 INCORRECT_TYPE, INDEX_OUT_OF_BOUNDS, NO_SUCH_FIELD, INVALID_JSON_POINTER = 17, 19, 20, 22
 NUMBER_OUT_OF_RANGE = 18
+NUMBER_ERROR = 9
 # kinds of sjb200_column_dev (SJB200_COLUMN_*)
 COLUMN_INT64, COLUMN_UINT64, COLUMN_BOOL, COLUMN_STRING, COLUMN_ARRAY_SIZE, COLUMN_OBJECT_SIZE = 1, 2, 3, 4, 5, 6
 DEPTH_ERROR = 4
@@ -266,6 +267,7 @@ def load():
         "sjb200_at_pointer_sharded_finish": (C.c_int, [vp, C.POINTER(ShardedPointerSummary)]),
         "sjb200_pointer_edge_fold": (C.c_int, [C.c_int, C.POINTER(PointerEdge), C.POINTER(PointerEdgeFoldResult), C.POINTER(PointerRank)]),
         "sjb200_column_dev": (C.c_int, [vp, C.c_int, vp, vp, C.c_uint32, vp, sz, vp, C.c_uint32, vp, vp, vp, vp, vp, sz, C.POINTER(ColumnResult), vp]),
+        "sjb200_column_double_dev": (C.c_int, [vp, vp, sz, vp, vp, vp, C.c_uint32, vp, C.c_uint32, vp, vp, vp, C.POINTER(ColumnResult), vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)

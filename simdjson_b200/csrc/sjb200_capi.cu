@@ -11,6 +11,7 @@
 
 #include "sjb200_bits.cuh"
 #include "sjb200_column.h"
+#include "sjb200_column_double.h"
 #include "sjb200_ctx.h"  // (with the CUDA runtime, include/sjb200.h and the launchers of sjb200_docs.cu and sjb200_tape.cu)
 #include "sjb200_finish.h"
 #include "sjb200_hostpipe.h"
@@ -889,6 +890,40 @@ extern "C" int sjb200_column_dev(sjb200_ctx *c, int kind, const uint8_t *d_type,
   out->rows_in_error = t.n_strings;
   if (str) out->string_bytes = t.string_bytes;
   return str && t.string_bytes > bytes_capacity ? SJB200_CAPACITY : SJB200_SUCCESS;
+}
+
+// element::get_double of every row of JSON Pointer results -- sjb200_column_double.cu
+extern "C" int sjb200_column_double_dev(sjb200_ctx *c, const uint8_t *d_buf, size_t len, const uint32_t *d_idx, const uint8_t *d_type,
+                                        const uint64_t *d_payload, uint32_t n, const sjb200_pointer_result *d_rows, uint32_t nrows, int32_t *d_err,
+                                        uint8_t *d_row_type, double *d_values, sjb200_column_result *out, void *stream) {
+  if (!c || !out) return SJB200_UNEXPECTED_ERROR;
+  out->rows_in_error = 0;
+  out->reserved = 0;
+  out->string_bytes = 0;
+  if ((n && (!d_type || !d_payload || !d_idx)) || (len && !d_buf) || (nrows && (!d_rows || !d_err || !d_row_type || !d_values))) return SJB200_UNEXPECTED_ERROR;
+  if (nrows == 0) return SJB200_SUCCESS;
+  static_assert(sizeof(sjb200_pointer_result) == sizeof(col::Row), "layout");
+  DeviceGuard g(c->device);
+  cudaStream_t s = stream_of(c, stream);
+  if (!grow(c, &c->d_col_scratch, &c->col_scratch_words, (dbl::column_double_scratch_bytes(nrows) + 7) / 8, "cudaMalloc(column scratch)")) return SJB200_MEMALLOC;
+  dbl::DoubleLaunch a{};
+  a.c = col::Cols{d_type, d_payload, n, nullptr, 0, reinterpret_cast<const col::Row *>(d_rows), nrows};
+  a.buf = d_buf;
+  a.len = len;
+  a.idx = d_idx;
+  a.err = d_err;
+  a.row_type = d_row_type;
+  a.values = reinterpret_cast<uint64_t *>(d_values);
+  uint32_t *counts = nullptr;
+  int launches = 0;
+  if (!ok(c, dbl::launch_column_double(a, c->d_col_scratch, &counts, c->sm_count, s, &launches), "column double") ||
+      !ok(c, cudaMemcpyAsync(c->h_small, counts, sizeof(uint32_t), cudaMemcpyDeviceToHost, s), "D2H column double totals") || !ok(c, cudaStreamSynchronize(s), "sync"))
+    return SJB200_UNEXPECTED_ERROR;
+  c->launches += launches;
+  uint32_t rows_in_error;
+  memcpy(&rows_in_error, c->h_small, sizeof(rows_in_error));
+  out->rows_in_error = rows_in_error;
+  return SJB200_SUCCESS;
 }
 
 // Stage-2 grammar over the stage-2-lite tokens (the error walk_document returns for every document) -- sjb200_grammar.cu

@@ -264,6 +264,31 @@ class dom_parser_implementation:
             raise RuntimeError(f"sjb200_column_dev: {capi.ERROR_NAMES.get(rc, rc)} {self.last_cuda_error()}")
         return e[:nrows].view(shape), t[:nrows].view(shape), vals[:nrows].view(shape)
 
+    def column_double_device(self, d_buf, d_type, d_payload, err, idx, d_idx=None, stream=None):
+        """element::get_double on every row of at_pointer_device's (err, idx), or of one pointer's row of them, on the
+        device (sjb200_column_double_dev): d_buf is the input of the stage-1 call whose structurals d_idx holds (default:
+        the buffer the last device-resident call wrote) and (d_type, d_payload) its tokens_device output.  Returns CUDA
+        tensors shaped like err: (error int32, row_type uint8, values float64), the correctly rounded double of each 'd',
+        'l' and 'u' row and +0.0 on an error.  A failure of the call raises."""
+        import torch
+        dev = d_type.device
+        shape = tuple(err.shape)
+        nrows = err.numel()
+        if d_idx is None:
+            d_idx = self.device_index_buffer()
+        rows = torch.stack((err.to(torch.int32), idx.to(torch.int32)), -1).to(dev).contiguous()
+        e = torch.empty(max(nrows, 1), dtype=torch.int32, device=dev)
+        t = torch.empty(max(nrows, 1), dtype=torch.uint8, device=dev)
+        v = torch.empty(max(nrows, 1), dtype=torch.float64, device=dev)
+        n = d_type.numel()
+        res = capi.ColumnResult()
+        rc = lib().sjb200_column_double_dev(self._ctx, d_buf.data_ptr() if d_buf.numel() else None, d_buf.numel(), d_idx.data_ptr() if n else None,
+                                            d_type.data_ptr() if n else None, d_payload.data_ptr() if n else None, n, rows.data_ptr() if nrows else None,
+                                            nrows, e.data_ptr(), t.data_ptr(), v.data_ptr(), C.byref(res), _stream_ptr(stream))
+        if rc != SUCCESS:
+            raise RuntimeError(f"sjb200_column_double_dev: {capi.ERROR_NAMES.get(rc, rc)} {self.last_cuda_error()}")
+        return e[:nrows].view(shape), t[:nrows].view(shape), v[:nrows].view(shape)
+
     def document_errors_device(self, d_type, d_payload, d_docs=None, ndocs=None, max_depth=None, stream=None):
         """the error stage 2 returns for every document (sjb200_document_errors_dev) over the output of tokens_device:
         d_docs = a document table (sjb200_document_table_dev, int32 pairs {index, byte}) and ndocs its entries in use, or
